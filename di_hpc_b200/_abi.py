@@ -141,25 +141,11 @@ def require_f32_cuda(name: str, t: torch.Tensor) -> torch.Tensor:
     return t.contiguous()
 
 
-def require_i64_cuda(name: str, t: torch.Tensor) -> torch.Tensor:
-    assert t.is_cuda, "%s must be a CUDA tensor (hpc version only supports cuda)" % name
-    if t.dtype != torch.int64:
-        raise TypeError("%s must be int64, got %s" % (name, t.dtype))
-    return t.contiguous()
-
-
 def workspace(op: int, T: int, B: int, N: int, device) -> torch.Tensor:
     """Allocate the scratch buffer an op asks for (torch caching allocator; stream-ordered reuse)."""
     with on_device(torch.device(device)):  # the size depends on the SM count of the tensor's device
         n = int(lib().hpc_rll_workspace_bytes(op, T, B, N))
     return torch.empty(max(n, 8), dtype=torch.uint8, device=device)
-
-
-def grad_scalar(g: torch.Tensor, like: torch.Tensor) -> torch.Tensor:
-    """Upstream gradient of a scalar loss as a 1-element fp32 device tensor (never read on the host)."""
-    if g is None:
-        return torch.zeros(1, dtype=torch.float32, device=like.device)
-    return g.reshape(1).to(dtype=torch.float32, device=like.device).contiguous()
 
 
 def launch_count() -> int:

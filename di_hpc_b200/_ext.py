@@ -1,10 +1,8 @@
 """Loader of the torch/pybind layer ``_lib/hpc_rl_utils_b200*.so`` (csrc_torch/: C++ autograd functions behind the
 nn.Modules, the reference's 30 ``hpc_rl_utils`` binding names, the padding list handling).
 
-Two bindings of the SAME CUDA library exist: this C++ layer (default; ~10x less host time per call) and the ctypes
-binding in ``_abi.py`` driven by the Python ``*Function`` classes.  ``HPC_RLL_BINDING=ctypes`` forces the latter (it is
-also what runs when the extension was built against a different torch).  Neither is a fallback in the sense of the
-product rules: both end in libhpc_rll_b200.so; without that library everything raises.
+The nn.Modules of ``rl_utils`` and the padding functions reach libhpc_rll_b200.so only through this extension; when it
+cannot be loaded, ``require()`` raises with the reason.
 """
 import glob
 import importlib.util
@@ -37,7 +35,7 @@ def load():
         spec.loader.exec_module(mod)
         sys.modules[_NAME] = mod
         _mod = mod
-    except Exception as e:  # noqa: BLE001  e.g. built against another torch: the ctypes binding still works
+    except Exception as e:  # noqa: BLE001  e.g. built against another torch: require() reports it
         _err = "%s: %s" % (type(e).__name__, e)
     return _mod
 
@@ -47,10 +45,7 @@ def why_missing():
 
 
 def fast():
-    """The extension if the C++ binding is selected and loadable, else None (callers then use the ctypes twin)."""
-    if os.environ.get("HPC_RLL_BINDING", "ext") == "ctypes":
-        return None
-    return load()
+    return load()  # kept for bench.py, which reports whether the extension loaded
 
 
 def require():
@@ -58,3 +53,10 @@ def require():
     if m is None:
         raise HpcRllError("torch extension %s unavailable: %s" % (_NAME, _err))
     return m
+
+
+def reference_function(apply):
+    """Decorator: a plain class named like ``apply`` whose static ``apply`` is the function, i.e. the reference's
+    ``*Function.apply`` entry point.  The autograd function behind it is the extension's C++ one (fast_ops.cpp)."""
+    return type(apply.__name__, (), {"apply": staticmethod(apply), "__module__": apply.__module__,
+                                     "__doc__": apply.__doc__})

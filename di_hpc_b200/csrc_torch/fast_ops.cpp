@@ -1,15 +1,11 @@
-// fast_ops.cpp -- the autograd layer of hpc_rll.rl_utils in C++ (round 2).
+// fast_ops.cpp -- the autograd layer of hpc_rll.rl_utils in C++.
 //
-// Round 1 bound the C ABI with ctypes underneath Python `torch.autograd.Function`s; that host path
-// cost tens of microseconds per forward+backward (argument checks, torch.empty, ctypes marshalling, Python autograd bookkeeping),
-// i.e. more than the kernels of the small ops (q_nstep_td, PPO, C51), and it
-// held the module-level GAE step measurably above the raw ABI.  Here the same
-// logic -- checks, output allocation, save-for-backward, the C-ABI call on PyTorch's current stream -- is one C++
-// `torch::autograd::Function` per op, and the nn.Modules of di_hpc_b200/rl_utils call straight into it.
-// The Python `*Function` classes stay (same names as /root/reference/hpc_rll/rl_utils/*.py) as the ctypes-bound
-// twins and are tested against these.
+// Argument checks, output allocation, save-for-backward and the C-ABI call on PyTorch's current stream are one C++
+// `torch::autograd::Function` per op; the nn.Modules of di_hpc_b200/rl_utils call straight into it through their
+// reference-named `*Function.apply`.  The same work in Python autograd + ctypes costs tens of microseconds of host time
+// per forward+backward, more than the kernels of the small ops (q_nstep_td, PPO, C51).
 //
-// Semantics, argument order and error behaviour follow di_hpc_b200/rl_utils/*.py one to one; nothing here computes.
+// Argument order follows the `*Function.apply` of di_hpc_b200/rl_utils/*.py; nothing here computes.
 #include "common.h"
 
 namespace hpcrl {
@@ -440,7 +436,7 @@ void register_fast_ops(pybind11::module& m) {
           "all-reduce(SUM) of <= 16 scalars over NVLink peer memory, differentiable (identity gradient)");
     namespace py = pybind11;
     m.def("gae", [](const Tensor& v, const Tensor& r, double g, double l) { return GaeFn::apply(v, r, g, l); },
-          "GAE forward with autograd (adjoint) -- C++ twin of GAEFunction");
+          "GAE forward with autograd (adjoint)");
     m.def("td_lambda",
           [](const Tensor& v, const Tensor& r, const OptTensor& w, double g, double l, int64_t gb) {
               return TdLambdaFn::apply(v, r, w, g, l, gb);

@@ -63,7 +63,7 @@ def gae_fwd_bwd_host(value, reward, grad_adv=None, gamma: float = 0.99, lambda_:
     """
     Overview:
         GAE forward (+ adjoint when ``grad_adv`` is given) on HOST tensors, pipelined through the current CUDA device.
-        Semantics of ``GAE.forward`` / ``GAEFunction.backward`` (hpc_rll/origin/gae.py:28-37), bit-identical to the
+        Semantics of ``GAE.forward`` and its backward (hpc_rll/origin/gae.py:28-37), bit-identical to the
         device-resident path.
     Arguments:
         - value (:obj:`torch.FloatTensor`): :math:`(T + 1, B)` CPU, contiguous (pinned memory for full copy speed)

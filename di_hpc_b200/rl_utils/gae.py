@@ -2,8 +2,8 @@
 
 Same constructor ``GAE(T, B)`` and ``forward(value, reward, gamma=0.99, lambda_=0.97)`` as the
 reference (gae.py:20-61).  Differences, all deliberate (DESIGN.md "Deviations"):
-  * ``GAEFunction.backward`` is a real adjoint (the reference returns None for every input,
-    gae.py:16-18, while hpc_rll/origin/gae.py is differentiable);
+  * the backward is a real adjoint (the reference's ``GAEFunction.backward`` returns None for every
+    input, gae.py:16-18, while hpc_rll/origin/gae.py is differentiable);
   * the result is a fresh tensor sized from the inputs, not the module-owned ``adv`` buffer returned
     by alias (gae.py:39,61) -- T and B of the constructor are kept only for API compatibility;
   * kernels run on PyTorch's current stream, with argument checks.
@@ -13,35 +13,9 @@ import torch
 from .. import _abi, _ext
 
 
-class GAEFunction(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, value, reward, gamma, lambda_):
-        value = _abi.require_f32_cuda("value", value)
-        reward = _abi.require_f32_cuda("reward", reward)
-        T, B = reward.shape
-        if value.shape != (T + 1, B):
-            raise ValueError("value must be (T+1, B)=(%d, %d), got %s" % (T + 1, B, tuple(value.shape)))
-        adv = torch.empty_like(reward)
-        with _abi.on_device(reward.device):
-            _abi.check(
-                _abi.lib().hpc_rll_gae_forward(_abi.ptr(value), _abi.ptr(reward), _abi.ptr(adv), T, B, float(gamma),
-                                               float(lambda_), _abi.stream_of(reward)), "hpc_rll_gae_forward")
-        ctx.gamma, ctx.lambda_, ctx.T, ctx.B = float(gamma), float(lambda_), T, B
-        return adv
-
-    @staticmethod
-    def backward(ctx, grad_adv):
-        T, B = ctx.T, ctx.B
-        grad_adv = _abi.require_f32_cuda("grad_adv", grad_adv)
-        grad_value = torch.empty((T + 1, B), dtype=torch.float32, device=grad_adv.device)
-        grad_reward = torch.empty((T, B), dtype=torch.float32, device=grad_adv.device)
-        with _abi.on_device(grad_adv.device):
-            _abi.check(
-                _abi.lib().hpc_rll_gae_backward(_abi.ptr(grad_adv), _abi.ptr(grad_value), _abi.ptr(grad_reward), T, B,
-                                                ctx.gamma, ctx.lambda_, _abi.stream_of(grad_adv)),
-                "hpc_rll_gae_backward")
-        return grad_value, grad_reward, None, None
+@_ext.reference_function
+def GAEFunction(value, reward, gamma, lambda_):
+    return _ext.require().gae(value, reward, float(gamma), float(lambda_))
 
 
 def gae_with_adv_stats(value, reward, gamma: float = 0.99, lambda_: float = 0.97, group=None):
@@ -117,7 +91,4 @@ class GAE(torch.nn.Module):
         """
         assert (value.is_cuda)
         assert (reward.is_cuda)
-        fast = _ext.fast()
-        if fast is not None:  # C++ autograd function (csrc_torch/fast_ops.cpp); GAEFunction is its ctypes-bound twin
-            return fast.gae(value, reward, float(gamma), float(lambda_))
         return GAEFunction.apply(value, reward, gamma, lambda_)

@@ -9,166 +9,42 @@ space (di_hpc_b200/csrc/padding.cu), so a call performs no cudaMalloc / cudaMemc
 to 7 of each per call, src/rl_utils/padding.cu:118-131,172-199).  UnPadding writes all outputs into one
 allocation and returns views of it (origin's default ``deepcopy=False`` also returns views).
 """
-import ctypes
-import itertools
 from functools import reduce
 from typing import List, Union
 
-import numpy as np
 import torch
 
-from .. import _abi
-
-_seed = itertools.count(0x5EED)
-_F32 = torch.float32
-
-
-from .. import _ext as _ext_loader
-
-_ext = _ext_loader.load()  # list handling in C++ (csrc_torch/ext.cpp); None -> same kernels through ctypes
+from .. import _ext
 
 
 def cum(t) -> int:
     return reduce(lambda x, y: x * y, t, 1)
 
 
-def _prepare(inputs, ndim):
-    """Validate once, return (contiguous tensors, shapes as an (n, ndim) int64 array)."""
-    assert len(inputs) > 0, "empty input list"
-    dev = inputs[0].device
-    assert dev.type == "cuda", "hpc version only supports cuda"
-    shapes = [t.shape for t in inputs]
-    if any(len(s) != ndim for s in shapes):
-        raise ValueError("expected %d-D tensors" % ndim)
-    if any(t.dtype is not _F32 for t in inputs):
-        raise TypeError("padding supports float32 tensors")
-    if any(t.device != dev for t in inputs):
-        raise ValueError("all tensors must live on one CUDA device")
-    if not all(t.is_contiguous() for t in inputs):
-        inputs = [t.contiguous() for t in inputs]
-    return list(inputs), np.array(shapes, dtype=np.int64).reshape(len(inputs), ndim)
-
-
-def _right3(a):
-    """(n, ndim) -> (n, 3) int32, right-aligned with leading ones."""
-    n, nd = a.shape
-    out = np.ones((n, 3), dtype=np.int32)
-    out[:, 3 - nd:] = a
-    return out
-
-
-def _ptr_table(ptrs):
-    return np.array(ptrs, dtype=np.uint64)
-
-
-def _pad_groups(inputs, shp, bounds, value):
-    """Pad inputs[bounds[g]:bounds[g+1]] to the max shape of group g -- one launch for all groups."""
-    dev = inputs[0].device
-    n, ndim = shp.shape
-    new_x, masks = [], []
-    dst = np.empty(n, dtype=np.uint64)
-    msk = np.empty(n, dtype=np.uint64)
-    padded = np.empty((n, ndim), dtype=np.int64)
-    for g in range(len(bounds) - 1):
-        lo, hi = bounds[g], bounds[g + 1]
-        mx = shp[lo:hi].max(axis=0)
-        full = (hi - lo, ) + tuple(int(v) for v in mx)
-        x = torch.empty(full, dtype=_F32, device=dev)
-        m = torch.empty(full, dtype=torch.int32, device=dev)
-        step = 4 * int(np.prod(mx))
-        idx = np.arange(hi - lo, dtype=np.uint64) * np.uint64(step)
-        dst[lo:hi] = np.uint64(x.data_ptr()) + idx
-        msk[lo:hi] = np.uint64(m.data_ptr()) + idx
-        padded[lo:hi] = mx
-        new_x.append(x)
-        masks.append(m)
-    src = _ptr_table([t.data_ptr() for t in inputs])
-    sh, pd = _right3(shp), _right3(padded)
-    with _abi.on_device(dev):
-        _abi.check(
-            _abi.lib().hpc_rll_pad_batch(src.ctypes.data, dst.ctypes.data, msk.ctypes.data, sh.ctypes.data,
-                                         pd.ctypes.data, n, int(value), _abi.stream_of(inputs[0])),
-            "hpc_rll_pad_batch")
-    return new_x, masks
-
-
-def _split(shp, group, group_mode):
-    n, ndim = shp.shape
-    shp = np.ascontiguousarray(shp)
-    L = _abi.lib()
-    if group_mode == 'oracle':
-        g = min(group, n)
-        pos = np.zeros(g + 1, dtype=np.int64)
-        _abi.check(L.hpc_rll_oracle_split_group(shp.ctypes.data, n, ndim, g, pos.ctypes.data), "oracle_split_group")
-        return pos.tolist()
-    starts = np.zeros(group + 2, dtype=np.int64)
-    cnt = ctypes.c_int(0)
-    _abi.check(
-        L.hpc_rll_sample_split_group(shp.ctypes.data, n, ndim, group, next(_seed), starts.ctypes.data,
-                                     ctypes.byref(cnt)), "sample_split_group")
-    return starts[:cnt.value + 1].tolist()
-
-
 def _padding(inputs, ndim, mode, value, group, group_mode):
     assert mode in ['constant'], mode
     assert group_mode in ['sample', 'oracle'], group_mode
     assert group >= 1, group
-    if _ext is not None and len(inputs) > 0 and inputs[0].is_cuda:
-        try:
-            if group > 1:
-                return _ext.group_pad_nd(list(inputs), ndim, group, 1 if group_mode == 'oracle' else 0, int(value))
-            new_x, mask, shapes = _ext.pad_nd(list(inputs), ndim, int(value))
-            return new_x, mask, shapes
-        except RuntimeError as e:  # TORCH_CHECK failures: map to the exception types of the ctypes path
-            msg = str(e)
-            if "float32" in msg:
-                raise TypeError(msg) from None
-            if "-D tensors" in msg or "one CUDA device" in msg:
-                raise ValueError(msg) from None
-            raise
-    inputs, shp = _prepare(inputs, ndim)
-    if group > 1:
-        order = np.argsort(shp.prod(axis=1), kind="stable")  # == sorted(key=numel), stable like Python's sort
-        inputs = [inputs[i] for i in order]
-        shp = shp[order]
-        bounds = _split(shp, group, group_mode)
-        new_x, mask = _pad_groups(inputs, shp, bounds, value)
-        shapes = [shp[bounds[g]:bounds[g + 1]].reshape(-1).tolist() for g in range(len(bounds) - 1)]
-        return [tuple(new_x), tuple(mask), tuple(shapes)]
-    new_x, mask = _pad_groups(inputs, shp, [0, len(inputs)], value)
-    return new_x[0], mask[0], shp.reshape(-1).tolist()
+    assert len(inputs) > 0, "empty input list"
+    assert inputs[0].is_cuda, "hpc version only supports cuda"
+    ext = _ext.require()  # list handling in C++ (csrc_torch/ext.cpp)
+    try:
+        if group > 1:
+            return ext.group_pad_nd(list(inputs), ndim, group, 1 if group_mode == 'oracle' else 0, int(value))
+        new_x, mask, shapes = ext.pad_nd(list(inputs), ndim, int(value))
+        return new_x, mask, shapes
+    except RuntimeError as e:  # ext.cpp's checks raise RuntimeError, which its Pad*Forward bindings keep
+        msg = str(e)
+        if "float32" in msg:
+            raise TypeError(msg) from None
+        if "-D tensors" in msg or "one CUDA device" in msg:
+            raise ValueError(msg) from None
+        raise
 
 
 def _unpad_one(x, shapes, ndim):
     assert x.is_cuda, "hpc version only supports cuda"
-    if _ext is not None:
-        return _ext.unpad_nd(x, [int(v) for v in shapes], ndim)
-    if x.dtype is not _F32:
-        raise TypeError("padding supports float32 tensors")
-    if not x.is_contiguous():
-        x = x.contiguous()
-    n = x.shape[0]
-    shp = np.asarray(shapes, dtype=np.int64)
-    if shp.size != n * ndim:
-        raise ValueError("shapes must hold %d ints per tensor" % ndim)
-    shp = shp.reshape(n, ndim)
-    sizes = shp.prod(axis=1)
-    flat = torch.empty(int(sizes.sum()), dtype=_F32, device=x.device)  # one allocation, outputs are views
-    offs = np.zeros(n, dtype=np.uint64)
-    np.cumsum(sizes[:-1], out=offs[1:].view(np.int64)) if n > 1 else None
-    dst = np.uint64(flat.data_ptr()) + offs * np.uint64(4)
-    vol = 4 * cum(x.shape[1:])
-    src = np.uint64(x.data_ptr()) + np.arange(n, dtype=np.uint64) * np.uint64(vol)
-    pad3 = _right3(np.broadcast_to(np.array(x.shape[1:], dtype=np.int64), (n, ndim)))
-    sh3 = _right3(shp)
-    with _abi.on_device(x.device):
-        _abi.check(
-            _abi.lib().hpc_rll_unpad_batch(src.ctypes.data, dst.ctypes.data, sh3.ctypes.data, pad3.ctypes.data, n,
-                                           _abi.stream_of(x)), "hpc_rll_unpad_batch")
-    pieces = flat.split(sizes.tolist())
-    if ndim == 1:
-        return list(pieces)
-    return [p.view(s) for p, s in zip(pieces, shp.tolist())]
+    return _ext.require().unpad_nd(x, [int(v) for v in shapes], ndim)
 
 
 def _unpadding(x, shapes, ndim):

@@ -8,7 +8,7 @@ from typing import Optional
 
 import torch
 
-from .. import _abi, _ext
+from .. import _ext
 
 hpc_ppo_loss = namedtuple('hpc_ppo_loss', ['policy_loss', 'value_loss', 'entropy_loss'])
 hpc_ppo_info = namedtuple('hpc_ppo_info', ['approx_kl', 'clipfrac'])
@@ -102,67 +102,12 @@ def _lazy_info(info):
     return hpc_ppo_info(LazyScalar(host, 0, ev), LazyScalar(host, 1, ev))
 
 
-class PPOFunction(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, logits_new, logits_old, action, value_new, value_old, adv, return_, weight, clip_ratio,
-                use_value_clip, dual_clip, global_B, adv_stats=None):
-        logits_new = _abi.require_f32_cuda("logits_new", logits_new)
-        logits_old = _abi.require_f32_cuda("logits_old", logits_old)
-        action = _abi.require_i64_cuda("action", action)
-        value_new = _abi.require_f32_cuda("value_new", value_new)
-        value_old = _abi.require_f32_cuda("value_old", value_old)
-        adv = _abi.require_f32_cuda("adv", adv)
-        return_ = _abi.require_f32_cuda("return_", return_)
-        B, N = logits_new.shape
-        if logits_old.shape != (B, N) or any(t.shape != (B, ) for t in (action, value_new, value_old, adv, return_)):
-            raise ValueError("ppo: inconsistent shapes")
-        if weight is not None:
-            weight = _abi.require_f32_cuda("weight", weight)
-            if weight.shape != (B, ):
-                raise ValueError("weight must be (B,)")
-        if adv_stats is not None:
-            adv_stats = _abi.require_f32_cuda("adv_stats", adv_stats)
-            if adv_stats.shape != (2, ):
-                raise ValueError("adv_stats must be (2,) = [mean, std + 1e-8]")
-        dev = adv.device
-        out = torch.empty(5, dtype=torch.float32, device=dev)
-        pol_coef = torch.empty(B, dtype=torch.float32, device=dev)
-        val_coef = torch.empty(B, dtype=torch.float32, device=dev)
-        ws = _abi.workspace(_abi.OP_PPO, 0, B, N, dev)
-        tail = (_abi.ptr(out), _abi.ptr(pol_coef), _abi.ptr(val_coef), B, N, float(clip_ratio),
-                1 if use_value_clip else 0, -1.0 if dual_clip is None else float(dual_clip), int(global_B),
-                _abi.ptr(ws), ws.numel(), _abi.stream_of(adv))
-        head = (_abi.ptr(logits_new), _abi.ptr(logits_old), _abi.ptr(action), _abi.ptr(value_new),
-                _abi.ptr(value_old), _abi.ptr(adv), _abi.ptr(return_), _abi.ptr(weight))
-        with _abi.on_device(dev):
-            if adv_stats is None:
-                _abi.check(_abi.lib().hpc_rll_ppo_forward(*head, *tail), "hpc_rll_ppo_forward")
-            else:
-                _abi.check(_abi.lib().hpc_rll_ppo_forward_norm(*head, _abi.ptr(adv_stats), *tail),
-                           "hpc_rll_ppo_forward_norm")
-        ctx.save_for_backward(logits_new, action, weight, pol_coef, val_coef)
-        ctx.global_B = int(global_B)
-        info = out[3:5]
-        ctx.mark_non_differentiable(info)
-        return out[0:1], out[1:2], out[2:3], info
-
-    @staticmethod
-    def backward(ctx, grad_policy_loss, grad_value_loss, grad_entropy_loss, grad_info):
-        logits_new, action, weight, pol_coef, val_coef = ctx.saved_tensors
-        B, N = logits_new.shape
-        g_p = _abi.grad_scalar(grad_policy_loss, pol_coef)
-        g_v = _abi.grad_scalar(grad_value_loss, pol_coef)
-        g_e = _abi.grad_scalar(grad_entropy_loss, pol_coef)
-        grad_logits = torch.empty_like(logits_new)
-        grad_value = torch.empty(B, dtype=torch.float32, device=pol_coef.device)
-        with _abi.on_device(pol_coef.device):
-            _abi.check(
-                _abi.lib().hpc_rll_ppo_backward(_abi.ptr(g_p), _abi.ptr(g_v), _abi.ptr(g_e), _abi.ptr(logits_new),
-                                                _abi.ptr(action), _abi.ptr(weight), _abi.ptr(pol_coef),
-                                                _abi.ptr(val_coef), _abi.ptr(grad_logits), _abi.ptr(grad_value), B, N,
-                                                ctx.global_B, _abi.stream_of(pol_coef)), "hpc_rll_ppo_backward")
-        return grad_logits, None, None, grad_value, None, None, None, None, None, None, None, None, None
+@_ext.reference_function
+def PPOFunction(logits_new, logits_old, action, value_new, value_old, adv, return_, weight, clip_ratio, use_value_clip,
+                dual_clip, global_B, adv_stats=None):
+    return tuple(_ext.require().ppo(logits_new, logits_old, action, value_new, value_old, adv, return_, weight,
+                                    float(clip_ratio), bool(use_value_clip),
+                                    -1.0 if dual_clip is None else float(dual_clip), int(global_B), adv_stats))
 
 
 class PPO(torch.nn.Module):
@@ -217,16 +162,10 @@ class PPO(torch.nn.Module):
             assert (weight.is_cuda)
         assert dual_clip is None or dual_clip > 1.0, \
             "dual_clip value must be greater than 1.0, but get value: {}".format(dual_clip)
-        fast = _ext.fast()
-        if fast is not None:
-            policy_loss, value_loss, entropy_loss, info = fast.ppo(
-                logits_new, logits_old, action, value_new, value_old, adv, return_, weight, float(clip_ratio),
-                bool(use_value_clip), -1.0 if dual_clip is None else float(dual_clip), int(self.global_B), adv_stats)
-        else:
-            policy_loss, value_loss, entropy_loss, info = PPOFunction.apply(logits_new, logits_old, action, value_new,
-                                                                            value_old, adv, return_, weight,
-                                                                            clip_ratio, use_value_clip, dual_clip,
-                                                                            self.global_B, adv_stats)
+        policy_loss, value_loss, entropy_loss, info = PPOFunction.apply(logits_new, logits_old, action, value_new,
+                                                                        value_old, adv, return_, weight, clip_ratio,
+                                                                        use_value_clip, dual_clip, self.global_B,
+                                                                        adv_stats)
         if self.lazy_info:
             return hpc_ppo_loss(policy_loss, value_loss, entropy_loss), _lazy_info(info)
         approx_kl, clipfrac = info.tolist()  # one device->host copy

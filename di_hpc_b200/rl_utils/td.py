@@ -18,68 +18,12 @@ from typing import Optional
 
 import torch
 
-from .. import _abi, _ext
+from .. import _ext
 
 
-def _nstep_common(q_like, action, next_n_action, reward, done, weight, B):
-    """Shared argument normalisation of the n-step family (reference asserts is_cuda only)."""
-    action = _abi.require_i64_cuda("action", action)
-    next_n_action = _abi.require_i64_cuda("next_n_action", next_n_action)
-    reward = _abi.require_f32_cuda("reward", reward)
-    if done.dtype != torch.float32:
-        # the reference kernels read `done` as float* (src/rl_utils/q_nstep_td.cu:39); accept bool too
-        done = done.to(torch.float32)
-    done = _abi.require_f32_cuda("done", done)
-    if action.shape != (B, ) or next_n_action.shape != (B, ) or done.shape != (B, ) or reward.dim() != 2 \
-            or reward.shape[1] != B:
-        raise ValueError("n-step td: inconsistent shapes (B=%d)" % B)
-    if weight is not None:
-        weight = _abi.require_f32_cuda("weight", weight)
-        if weight.shape != (B, ):
-            raise ValueError("weight must be (B,)")
-    return action, next_n_action, reward, done, weight
-
-
-class TDLambdaFunction(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, value, reward, weight, gamma, lambda_, global_B):
-        value = _abi.require_f32_cuda("value", value)
-        reward = _abi.require_f32_cuda("reward", reward)
-        T, B = reward.shape
-        if value.shape != (T + 1, B):
-            raise ValueError("value must be (T+1, B)=(%d, %d), got %s" % (T + 1, B, tuple(value.shape)))
-        if weight is not None:
-            weight = _abi.require_f32_cuda("weight", weight)
-            if weight.dim() == 1:
-                # the reference documents weight as (B,) (td.py:172) though its kernel indexes (T,B)
-                # (td_lambda_kernel.h:24); broadcast the documented form
-                weight = weight.unsqueeze(0).expand(T, B).contiguous()
-            if weight.shape != (T, B):
-                raise ValueError("weight must be (T, B) or (B,), got %s" % (tuple(weight.shape),))
-        loss = torch.empty(1, dtype=torch.float32, device=reward.device)
-        grad_buf = torch.empty_like(reward)
-        ws = _abi.workspace(_abi.OP_TD_LAMBDA, T, B, 0, reward.device)
-        with _abi.on_device(reward.device):
-            _abi.check(
-                _abi.lib().hpc_rll_td_lambda_forward(_abi.ptr(value), _abi.ptr(reward), _abi.ptr(weight),
-                                                     _abi.ptr(loss), _abi.ptr(grad_buf), T, B, float(gamma),
-                                                     float(lambda_), int(global_B), _abi.ptr(ws), ws.numel(),
-                                                     _abi.stream_of(reward)), "hpc_rll_td_lambda_forward")
-        ctx.save_for_backward(grad_buf)
-        return loss
-
-    @staticmethod
-    def backward(ctx, grad_loss):
-        (grad_buf, ) = ctx.saved_tensors
-        T, B = grad_buf.shape
-        g = _abi.grad_scalar(grad_loss, grad_buf)
-        grad_value = torch.empty((T + 1, B), dtype=torch.float32, device=grad_buf.device)
-        with _abi.on_device(grad_buf.device):
-            _abi.check(
-                _abi.lib().hpc_rll_td_lambda_backward(_abi.ptr(g), _abi.ptr(grad_buf), _abi.ptr(grad_value), T, B,
-                                                      _abi.stream_of(grad_buf)), "hpc_rll_td_lambda_backward")
-        return grad_value, None, None, None, None, None
+@_ext.reference_function
+def TDLambdaFunction(value, reward, weight, gamma, lambda_, global_B):
+    return _ext.require().td_lambda(value, reward, weight, float(gamma), float(lambda_), int(global_B))
 
 
 class TDLambda(torch.nn.Module):
@@ -116,80 +60,20 @@ class TDLambda(torch.nn.Module):
         assert (reward.is_cuda)
         if weight is not None:
             assert (weight.is_cuda)
-        fast = _ext.fast()
-        if fast is not None:
-            return fast.td_lambda(value, reward, weight, float(gamma), float(lambda_), int(self.global_B))
         return TDLambdaFunction.apply(value, reward, weight, gamma, lambda_, self.global_B)
 
 
 # ------------------------------------------------------------------------------------------- q n-step
-class _QNStepTDBase(torch.autograd.Function):
-    RESCALE = 0
-
-    @classmethod
-    def _fwd(cls, ctx, q, next_n_q, action, next_n_action, reward, done, weight, gamma, global_B):
-        q = _abi.require_f32_cuda("q", q)
-        next_n_q = _abi.require_f32_cuda("next_n_q", next_n_q)
-        B, N = q.shape
-        if next_n_q.shape != (B, N):
-            raise ValueError("next_n_q must match q")
-        action, next_n_action, reward, done, weight = _nstep_common(q, action, next_n_action, reward, done, weight, B)
-        T = reward.shape[0]
-        dev = q.device
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        td_err = torch.empty(B, dtype=torch.float32, device=dev)
-        grad_buf = torch.empty(B, dtype=torch.float32, device=dev)
-        ws = _abi.workspace(_abi.OP_Q_NSTEP_TD, T, B, N, dev)
-        with _abi.on_device(dev):
-            _abi.check(
-                _abi.lib().hpc_rll_q_nstep_td_forward(_abi.ptr(q), _abi.ptr(next_n_q), _abi.ptr(action),
-                                                      _abi.ptr(next_n_action), _abi.ptr(reward), _abi.ptr(done),
-                                                      _abi.ptr(weight), _abi.ptr(loss), _abi.ptr(td_err),
-                                                      _abi.ptr(grad_buf), T, B, N, float(gamma), cls.RESCALE,
-                                                      int(global_B), _abi.ptr(ws), ws.numel(), _abi.stream_of(q)),
-                "hpc_rll_q_nstep_td_forward")
-        ctx.save_for_backward(grad_buf, action)
-        ctx.N = N
-        ctx.mark_non_differentiable(td_err)
-        return loss, td_err
-
-    @staticmethod
-    def _bwd(ctx, grad_loss):
-        grad_buf, action = ctx.saved_tensors
-        B, N = grad_buf.shape[0], ctx.N
-        g = _abi.grad_scalar(grad_loss, grad_buf)
-        grad_q = torch.empty((B, N), dtype=torch.float32, device=grad_buf.device)
-        with _abi.on_device(grad_buf.device):
-            _abi.check(
-                _abi.lib().hpc_rll_q_nstep_td_backward(_abi.ptr(g), _abi.ptr(grad_buf), _abi.ptr(action),
-                                                       _abi.ptr(grad_q), B, N, _abi.stream_of(grad_buf)),
-                "hpc_rll_q_nstep_td_backward")
-        return grad_q
+@_ext.reference_function
+def QNStepTDFunction(q, next_n_q, action, next_n_action, reward, done, weight, gamma, global_B):
+    return tuple(_ext.require().q_nstep_td(q, next_n_q, action, next_n_action, reward, done, weight, float(gamma),
+                                           False, int(global_B)))
 
 
-class QNStepTDFunction(_QNStepTDBase):
-    RESCALE = 0
-
-    @staticmethod
-    def forward(ctx, q, next_n_q, action, next_n_action, reward, done, weight, gamma, global_B):
-        return QNStepTDFunction._fwd(ctx, q, next_n_q, action, next_n_action, reward, done, weight, gamma, global_B)
-
-    @staticmethod
-    def backward(ctx, grad_loss, grad_td_err):
-        return (_QNStepTDBase._bwd(ctx, grad_loss), ) + (None, ) * 8
-
-
-class QNStepTDRescaleFunction(_QNStepTDBase):
-    RESCALE = 1
-
-    @staticmethod
-    def forward(ctx, q, next_n_q, action, next_n_action, reward, done, weight, gamma, global_B):
-        return QNStepTDRescaleFunction._fwd(ctx, q, next_n_q, action, next_n_action, reward, done, weight, gamma,
-                                            global_B)
-
-    @staticmethod
-    def backward(ctx, grad_loss, grad_td_err):
-        return (_QNStepTDBase._bwd(ctx, grad_loss), ) + (None, ) * 8
+@_ext.reference_function
+def QNStepTDRescaleFunction(q, next_n_q, action, next_n_action, reward, done, weight, gamma, global_B):
+    return tuple(_ext.require().q_nstep_td(q, next_n_q, action, next_n_action, reward, done, weight, float(gamma),
+                                           True, int(global_B)))
 
 
 class QNStepTD(torch.nn.Module):
@@ -231,10 +115,6 @@ class QNStepTD(torch.nn.Module):
             assert (t.is_cuda)
         if weight is not None:
             assert (weight.is_cuda)
-        fast = _ext.fast()
-        if fast is not None:
-            return tuple(fast.q_nstep_td(q, next_n_q, action, next_n_action, reward, done, weight, float(gamma),
-                                         bool(self._fn.RESCALE), int(self.global_B)))
         return self._fn.apply(q, next_n_q, action, next_n_action, reward, done, weight, gamma, self.global_B)
 
 
@@ -247,50 +127,10 @@ class QNStepTDRescale(QNStepTD):
 
 
 # ------------------------------------------------------------------------------------------- C51
-class DistNStepTDFunction(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, dist, next_n_dist, action, next_n_action, reward, done, weight, gamma, v_min, v_max, global_B):
-        dist = _abi.require_f32_cuda("dist", dist)
-        next_n_dist = _abi.require_f32_cuda("next_n_dist", next_n_dist)
-        B, N, n_atom = dist.shape
-        if next_n_dist.shape != (B, N, n_atom):
-            raise ValueError("next_n_dist must match dist")
-        action, next_n_action, reward, done, weight = _nstep_common(dist, action, next_n_action, reward, done, weight,
-                                                                    B)
-        T = reward.shape[0]
-        dev = dist.device
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        td_err = torch.empty(B, dtype=torch.float32, device=dev)
-        grad_buf = torch.empty((B, n_atom), dtype=torch.float32, device=dev)
-        ws = _abi.workspace(_abi.OP_DIST_NSTEP_TD, T, B, N, dev)
-        with _abi.on_device(dev):
-            _abi.check(
-                _abi.lib().hpc_rll_dist_nstep_td_forward(_abi.ptr(dist), _abi.ptr(next_n_dist), _abi.ptr(action),
-                                                         _abi.ptr(next_n_action), _abi.ptr(reward), _abi.ptr(done),
-                                                         _abi.ptr(weight), _abi.ptr(loss), _abi.ptr(td_err),
-                                                         _abi.ptr(grad_buf), T, B, N, n_atom, float(gamma),
-                                                         float(v_min), float(v_max), int(global_B), _abi.ptr(ws),
-                                                         ws.numel(), _abi.stream_of(dist)),
-                "hpc_rll_dist_nstep_td_forward")
-        ctx.save_for_backward(grad_buf, action)
-        ctx.N = N
-        ctx.mark_non_differentiable(td_err)
-        return loss, td_err
-
-    @staticmethod
-    def backward(ctx, grad_loss, grad_td_err):
-        grad_buf, action = ctx.saved_tensors
-        B, n_atom = grad_buf.shape
-        N = ctx.N
-        g = _abi.grad_scalar(grad_loss, grad_buf)
-        grad_dist = torch.empty((B, N, n_atom), dtype=torch.float32, device=grad_buf.device)
-        with _abi.on_device(grad_buf.device):
-            _abi.check(
-                _abi.lib().hpc_rll_dist_nstep_td_backward(_abi.ptr(g), _abi.ptr(grad_buf), _abi.ptr(action),
-                                                          _abi.ptr(grad_dist), B, N, n_atom,
-                                                          _abi.stream_of(grad_buf)), "hpc_rll_dist_nstep_td_backward")
-        return (grad_dist, ) + (None, ) * 10
+@_ext.reference_function
+def DistNStepTDFunction(dist, next_n_dist, action, next_n_action, reward, done, weight, gamma, v_min, v_max, global_B):
+    return tuple(_ext.require().dist_nstep_td(dist, next_n_dist, action, next_n_action, reward, done, weight,
+                                              float(gamma), float(v_min), float(v_max), int(global_B)))
 
 
 class DistNStepTD(torch.nn.Module):
@@ -338,61 +178,15 @@ class DistNStepTD(torch.nn.Module):
         if self.check_positive:
             batch_range = torch.arange(action.shape[0], device=action.device)
             assert (dist[batch_range, action] > 0.0).all(), ("dist act", dist[batch_range, action], "dist:", dist)
-        fast = _ext.fast()
-        if fast is not None:
-            return tuple(fast.dist_nstep_td(dist, next_n_dist, action, next_n_action, reward, done, weight,
-                                            float(gamma), float(v_min), float(v_max), int(self.global_B)))
         return DistNStepTDFunction.apply(dist, next_n_dist, action, next_n_action, reward, done, weight, gamma, v_min,
                                          v_max, self.global_B)
 
 
 # ------------------------------------------------------------------------------------------- QR-DQN
-class QRDQNNStepTDErrorFunction(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, gamma, global_B):
-        q = _abi.require_f32_cuda("q", q)
-        next_n_q = _abi.require_f32_cuda("next_n_q", next_n_q)
-        B, N, tau = q.shape
-        if next_n_q.shape != (B, N, tau):
-            raise ValueError("next_n_q must match q")
-        action, next_n_action, reward, done, weight = _nstep_common(q, action, next_n_action, reward, done, weight, B)
-        if value_gamma is not None:
-            value_gamma = _abi.require_f32_cuda("value_gamma", value_gamma)
-            if value_gamma.shape != (B, ):
-                raise ValueError("value_gamma must be (B,)")
-        T = reward.shape[0]
-        dev = q.device
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        td_err = torch.empty(B, dtype=torch.float32, device=dev)
-        grad_buf = torch.empty((B, tau), dtype=torch.float32, device=dev)
-        ws = _abi.workspace(_abi.OP_QRDQN_NSTEP_TD, T, B, N, dev)
-        with _abi.on_device(dev):
-            _abi.check(
-                _abi.lib().hpc_rll_qrdqn_nstep_td_forward(_abi.ptr(q), _abi.ptr(next_n_q), _abi.ptr(action),
-                                                          _abi.ptr(next_n_action), _abi.ptr(reward), _abi.ptr(done),
-                                                          _abi.ptr(weight), _abi.ptr(value_gamma), _abi.ptr(loss),
-                                                          _abi.ptr(td_err), _abi.ptr(grad_buf), tau, T, B, N,
-                                                          float(gamma), int(global_B), _abi.ptr(ws), ws.numel(),
-                                                          _abi.stream_of(q)), "hpc_rll_qrdqn_nstep_td_forward")
-        ctx.save_for_backward(grad_buf, action)
-        ctx.N = N
-        ctx.mark_non_differentiable(td_err)
-        return loss, td_err
-
-    @staticmethod
-    def backward(ctx, grad_loss, grad_td_err):
-        grad_buf, action = ctx.saved_tensors
-        B, tau = grad_buf.shape
-        N = ctx.N
-        g = _abi.grad_scalar(grad_loss, grad_buf)
-        grad_q = torch.empty((B, N, tau), dtype=torch.float32, device=grad_buf.device)
-        with _abi.on_device(grad_buf.device):
-            _abi.check(
-                _abi.lib().hpc_rll_qrdqn_nstep_td_backward(_abi.ptr(g), _abi.ptr(grad_buf), _abi.ptr(action),
-                                                           _abi.ptr(grad_q), tau, B, N, _abi.stream_of(grad_buf)),
-                "hpc_rll_qrdqn_nstep_td_backward")
-        return (grad_q, ) + (None, ) * 9
+@_ext.reference_function
+def QRDQNNStepTDErrorFunction(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, gamma, global_B):
+    return tuple(_ext.require().qrdqn_nstep_td(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma,
+                                               float(gamma), int(global_B)))
 
 
 class QRDQNNStepTDError(torch.nn.Module):
@@ -437,67 +231,16 @@ class QRDQNNStepTDError(torch.nn.Module):
             assert (weight.is_cuda)
         if value_gamma is not None:
             assert (value_gamma.is_cuda)
-        fast = _ext.fast()
-        if fast is not None:
-            return tuple(fast.qrdqn_nstep_td(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma,
-                                             float(gamma), int(self.global_B)))
         return QRDQNNStepTDErrorFunction.apply(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma,
                                                gamma, self.global_B)
 
 
 # ------------------------------------------------------------------------------------------- IQN
-class IQNNStepTDErrorFunction(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, q, next_n_q, action, next_n_action, reward, done, replay_quantiles, weight, value_gamma, gamma,
-                kappa, global_B):
-        q = _abi.require_f32_cuda("q", q)
-        next_n_q = _abi.require_f32_cuda("next_n_q", next_n_q)
-        replay_quantiles = _abi.require_f32_cuda("replay_quantiles", replay_quantiles)
-        tau, B, N = q.shape
-        tau_p = next_n_q.shape[0]
-        if next_n_q.shape != (tau_p, B, N):
-            raise ValueError("next_n_q must be (tau', B, N)")
-        if replay_quantiles.numel() != tau * B:
-            raise ValueError("replay_quantiles must hold tau*B values")
-        action, next_n_action, reward, done, weight = _nstep_common(q, action, next_n_action, reward, done, weight, B)
-        if value_gamma is not None:
-            value_gamma = _abi.require_f32_cuda("value_gamma", value_gamma)
-            if value_gamma.shape != (B, ):
-                raise ValueError("value_gamma must be (B,)")
-        T = reward.shape[0]
-        dev = q.device
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        td_err = torch.empty(B, dtype=torch.float32, device=dev)
-        grad_buf = torch.empty((tau, B), dtype=torch.float32, device=dev)
-        ws = _abi.workspace(_abi.OP_IQN_NSTEP_TD, T, B, N, dev)
-        with _abi.on_device(dev):
-            _abi.check(
-                _abi.lib().hpc_rll_iqn_nstep_td_forward(_abi.ptr(q), _abi.ptr(next_n_q), _abi.ptr(action),
-                                                        _abi.ptr(next_n_action), _abi.ptr(reward), _abi.ptr(done),
-                                                        _abi.ptr(replay_quantiles), _abi.ptr(weight),
-                                                        _abi.ptr(value_gamma), _abi.ptr(loss), _abi.ptr(td_err),
-                                                        _abi.ptr(grad_buf), tau, tau_p, T, B, N, float(gamma),
-                                                        float(kappa), int(global_B), _abi.ptr(ws), ws.numel(),
-                                                        _abi.stream_of(q)), "hpc_rll_iqn_nstep_td_forward")
-        ctx.save_for_backward(grad_buf, action)
-        ctx.N = N
-        ctx.mark_non_differentiable(td_err)
-        return loss, td_err
-
-    @staticmethod
-    def backward(ctx, grad_loss, grad_td_err):
-        grad_buf, action = ctx.saved_tensors
-        tau, B = grad_buf.shape
-        N = ctx.N
-        g = _abi.grad_scalar(grad_loss, grad_buf)
-        grad_q = torch.empty((tau, B, N), dtype=torch.float32, device=grad_buf.device)
-        with _abi.on_device(grad_buf.device):
-            _abi.check(
-                _abi.lib().hpc_rll_iqn_nstep_td_backward(_abi.ptr(g), _abi.ptr(grad_buf), _abi.ptr(action),
-                                                         _abi.ptr(grad_q), tau, B, N, _abi.stream_of(grad_buf)),
-                "hpc_rll_iqn_nstep_td_backward")
-        return (grad_q, ) + (None, ) * 11
+@_ext.reference_function
+def IQNNStepTDErrorFunction(q, next_n_q, action, next_n_action, reward, done, replay_quantiles, weight, value_gamma,
+                            gamma, kappa, global_B):
+    return tuple(_ext.require().iqn_nstep_td(q, next_n_q, action, next_n_action, reward, done, replay_quantiles,
+                                             weight, value_gamma, float(gamma), float(kappa), int(global_B)))
 
 
 class IQNNStepTDError(torch.nn.Module):
@@ -544,9 +287,5 @@ class IQNNStepTDError(torch.nn.Module):
             assert (weight.is_cuda)
         if value_gamma is not None:
             assert (value_gamma.is_cuda)
-        fast = _ext.fast()
-        if fast is not None:
-            return tuple(fast.iqn_nstep_td(q, next_n_q, action, next_n_action, reward, done, replay_quantiles, weight,
-                                           value_gamma, float(gamma), float(kappa), int(self.global_B)))
         return IQNNStepTDErrorFunction.apply(q, next_n_q, action, next_n_action, reward, done, replay_quantiles,
                                              weight, value_gamma, gamma, kappa, self.global_B)

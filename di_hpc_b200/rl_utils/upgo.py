@@ -3,46 +3,12 @@ Same constructor ``UPGO(T, B, N)`` and ``forward(target_output, rhos, action, re
 bootstrap_values)`` (upgo.py:46-79); the loss is a shape-(1,) tensor."""
 import torch
 
-from .. import _abi, _ext
+from .. import _ext
 
 
-class UpgoFunction(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, target_output, rho, action, reward, value, global_B):
-        target_output = _abi.require_f32_cuda("target_output", target_output)
-        rho = _abi.require_f32_cuda("rhos", rho)
-        action = _abi.require_i64_cuda("action", action)
-        reward = _abi.require_f32_cuda("rewards", reward)
-        value = _abi.require_f32_cuda("bootstrap_values", value)
-        T, B, N = target_output.shape
-        if rho.shape != (T, B) or action.shape != (T, B) or reward.shape != (T, B) or value.shape != (T + 1, B):
-            raise ValueError("upgo: inconsistent shapes")
-        dev = reward.device
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        coef = torch.empty((T, B), dtype=torch.float32, device=dev)
-        ws = _abi.workspace(_abi.OP_UPGO, T, B, N, dev)
-        with _abi.on_device(dev):
-            _abi.check(
-                _abi.lib().hpc_rll_upgo_forward(_abi.ptr(target_output), _abi.ptr(rho), _abi.ptr(action),
-                                                _abi.ptr(reward), _abi.ptr(value), _abi.ptr(loss), _abi.ptr(coef), T,
-                                                B, N, int(global_B), _abi.ptr(ws), ws.numel(),
-                                                _abi.stream_of(reward)), "hpc_rll_upgo_forward")
-        ctx.save_for_backward(target_output, action, coef)
-        return loss
-
-    @staticmethod
-    def backward(ctx, grad_loss):
-        target_output, action, coef = ctx.saved_tensors
-        T, B, N = target_output.shape
-        g = _abi.grad_scalar(grad_loss, coef)
-        grad_target = torch.empty_like(target_output)
-        with _abi.on_device(coef.device):
-            _abi.check(
-                _abi.lib().hpc_rll_upgo_backward(_abi.ptr(g), _abi.ptr(target_output), _abi.ptr(action),
-                                                 _abi.ptr(coef), _abi.ptr(grad_target), T, B, N,
-                                                 _abi.stream_of(coef)), "hpc_rll_upgo_backward")
-        return grad_target, None, None, None, None, None
+@_ext.reference_function
+def UpgoFunction(target_output, rho, action, reward, value, global_B):
+    return _ext.require().upgo(target_output, rho, action, reward, value, int(global_B))
 
 
 class UPGO(torch.nn.Module):
@@ -81,7 +47,4 @@ class UPGO(torch.nn.Module):
         assert (action.is_cuda)
         assert (rewards.is_cuda)
         assert (bootstrap_values.is_cuda)
-        fast = _ext.fast()
-        if fast is not None:
-            return fast.upgo(target_output, rhos, action, rewards, bootstrap_values, int(self.global_B))
         return UpgoFunction.apply(target_output, rhos, action, rewards, bootstrap_values, self.global_B)

@@ -5,63 +5,17 @@ from collections import namedtuple
 
 import torch
 
-from .. import _abi, _ext
+from .. import _ext
 
 hpc_vtrace_loss = namedtuple('hpc_vtrace_loss', ['policy_loss', 'value_loss', 'entropy_loss'])
 
 
-class VtraceFunction(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, target_output, behaviour_output, action, value, reward, weight, gamma, lambda_, rho_clip_ratio,
-                c_clip_ratio, rho_pg_clip_ratio, global_B):
-        target_output = _abi.require_f32_cuda("target_output", target_output)
-        behaviour_output = _abi.require_f32_cuda("behaviour_output", behaviour_output)
-        action = _abi.require_i64_cuda("action", action)
-        value = _abi.require_f32_cuda("value", value)
-        reward = _abi.require_f32_cuda("reward", reward)
-        T, B, N = target_output.shape
-        if behaviour_output.shape != (T, B, N) or action.shape != (T, B) or reward.shape != (T, B) \
-                or value.shape != (T + 1, B):
-            raise ValueError("vtrace: inconsistent shapes")
-        if weight is not None:
-            weight = _abi.require_f32_cuda("weight", weight)
-            if weight.shape != (T, B):
-                raise ValueError("weight must be (T, B)")
-        dev = reward.device
-        losses = torch.empty(3, dtype=torch.float32, device=dev)
-        pg_coef = torch.empty((T, B), dtype=torch.float32, device=dev)
-        gv_buf = torch.empty((T, B), dtype=torch.float32, device=dev)
-        ws = _abi.workspace(_abi.OP_VTRACE, T, B, N, dev)
-        with _abi.on_device(dev):
-            _abi.check(
-                _abi.lib().hpc_rll_vtrace_forward(
-                    _abi.ptr(target_output), _abi.ptr(behaviour_output), _abi.ptr(action), _abi.ptr(value),
-                    _abi.ptr(reward), _abi.ptr(weight), _abi.ptr(losses), _abi.ptr(pg_coef), _abi.ptr(gv_buf), T, B, N,
-                    float(gamma), float(lambda_), float(rho_clip_ratio), float(c_clip_ratio),
-                    float(rho_pg_clip_ratio), int(global_B), _abi.ptr(ws), ws.numel(), _abi.stream_of(reward)),
-                "hpc_rll_vtrace_forward")
-        ctx.save_for_backward(target_output, action, weight, pg_coef, gv_buf)
-        ctx.global_B = int(global_B)
-        return losses[0:1], losses[1:2], losses[2:3]
-
-    @staticmethod
-    def backward(ctx, grad_pg_loss, grad_value_loss, grad_entropy_loss):
-        target_output, action, weight, pg_coef, gv_buf = ctx.saved_tensors
-        T, B, N = target_output.shape
-        g_pg = _abi.grad_scalar(grad_pg_loss, pg_coef)
-        g_v = _abi.grad_scalar(grad_value_loss, pg_coef)
-        g_e = _abi.grad_scalar(grad_entropy_loss, pg_coef)
-        grad_target = torch.empty_like(target_output)
-        grad_value = torch.empty((T + 1, B), dtype=torch.float32, device=pg_coef.device)
-        with _abi.on_device(pg_coef.device):
-            _abi.check(
-                _abi.lib().hpc_rll_vtrace_backward(_abi.ptr(g_pg), _abi.ptr(g_v), _abi.ptr(g_e),
-                                                   _abi.ptr(target_output), _abi.ptr(action), _abi.ptr(weight),
-                                                   _abi.ptr(pg_coef), _abi.ptr(gv_buf), _abi.ptr(grad_target),
-                                                   _abi.ptr(grad_value), T, B, N, ctx.global_B,
-                                                   _abi.stream_of(pg_coef)), "hpc_rll_vtrace_backward")
-        return grad_target, None, None, grad_value, None, None, None, None, None, None, None, None
+@_ext.reference_function
+def VtraceFunction(target_output, behaviour_output, action, value, reward, weight, gamma, lambda_, rho_clip_ratio,
+                   c_clip_ratio, rho_pg_clip_ratio, global_B):
+    return tuple(_ext.require().vtrace(target_output, behaviour_output, action, value, reward, weight, float(gamma),
+                                       float(lambda_), float(rho_clip_ratio), float(c_clip_ratio),
+                                       float(rho_pg_clip_ratio), int(global_B)))
 
 
 class VTrace(torch.nn.Module):
@@ -105,12 +59,6 @@ class VTrace(torch.nn.Module):
         assert (reward.is_cuda)
         if weight is not None:
             assert (weight.is_cuda)
-        fast = _ext.fast()
-        if fast is not None:
-            return hpc_vtrace_loss(*fast.vtrace(target_output, behaviour_output, action, value, reward, weight,
-                                                float(gamma), float(lambda_), float(rho_clip_ratio),
-                                                float(c_clip_ratio), float(rho_pg_clip_ratio), int(self.global_B)))
-        pg_loss, value_loss, entropy_loss = VtraceFunction.apply(target_output, behaviour_output, action, value,
-                                                                 reward, weight, gamma, lambda_, rho_clip_ratio,
-                                                                 c_clip_ratio, rho_pg_clip_ratio, self.global_B)
-        return hpc_vtrace_loss(pg_loss, value_loss, entropy_loss)
+        return hpc_vtrace_loss(*VtraceFunction.apply(target_output, behaviour_output, action, value, reward, weight,
+                                                     gamma, lambda_, rho_clip_ratio, c_clip_ratio, rho_pg_clip_ratio,
+                                                     self.global_B))

@@ -100,17 +100,6 @@ class P2PScalarAllReduce:
             self._local = None
 
 
-class _AllReduceSumP2P(torch.autograd.Function):
-
-    @staticmethod
-    def forward(ctx, x, comm):
-        return comm(x.detach().to(torch.float32).contiguous().clone())
-
-    @staticmethod
-    def backward(ctx, g):
-        return g, None
-
-
 _default_comm: Optional[P2PScalarAllReduce] = None
 
 
@@ -131,11 +120,7 @@ def all_reduce_losses(losses: Sequence[torch.Tensor], group=None, comm: Optional
     flat = losses[0].reshape(-1) if len(losses) == 1 else torch.cat([l.reshape(-1) for l in losses])
     comm = comm if comm is not None else _default_comm
     if comm is not None and flat.is_cuda and flat.numel() <= 16:
-        fast = _ext.fast()
-        if fast is not None and hasattr(fast, "allreduce_scalars_p2p"):  # C++ autograd function: no Python bookkeeping
-            red = fast.allreduce_scalars_p2p(flat, ctypes.addressof(comm._bufs), comm.rank, comm.world)
-        else:
-            red = _AllReduceSumP2P.apply(flat, comm)
+        red = _ext.require().allreduce_scalars_p2p(flat, ctypes.addressof(comm._bufs), comm.rank, comm.world)
     else:
         red = _AllReduceSum.apply(flat, group)
     out, o = [], 0

@@ -115,8 +115,8 @@ def test_reference_named_pybind_bindings():
     """The thin torch/pybind layer exports the reference's 11 padding bindings (src/rl_utils/entry.cpp:9-20)
     with the same call conventions as hpc_rll/rl_utils/padding.py uses them."""
     need_cuda()
-    import di_hpc_b200.rl_utils.padding as P
-    E = P._ext
+    from di_hpc_b200 import _ext
+    E = _ext.require()
     assert E is not None, "hpc_rl_utils_b200 extension missing (python -m di_hpc_b200.build_torch_ext)"
     rng = np.random.default_rng(3)
     shapes = [(int(rng.integers(3, 9)), int(rng.integers(2, 7))) for _ in range(20)]
