@@ -10,6 +10,7 @@ The package holds only what that path needs:
   rl_utils/   host-side mirror of the reference's `hpc_rll.rl_utils` modules (same class names,
               constructor arguments and forward signatures); `hpc_rll/` at the repo root re-exports it
               under the reference's import paths so DI-engine can swap it in unchanged.
+  torch_utils/ the same for `hpc_rll.torch_utils.network.scatter_connection` (ScatterConnection; no LSTM).
 There is no CPU fallback and no multi-backend dispatch.
 """
 __version__ = "0.1.0"

@@ -1,11 +1,12 @@
-// fast_ops.cpp -- the autograd layer of hpc_rll.rl_utils in C++.
+// fast_ops.cpp -- the autograd layer of hpc_rll.rl_utils and hpc_rll.torch_utils in C++.
 //
 // Argument checks, output allocation, save-for-backward and the C-ABI call on PyTorch's current stream are one C++
 // `torch::autograd::Function` per op; the nn.Modules of di_hpc_b200/rl_utils call straight into it through their
 // reference-named `*Function.apply`.  The same work in Python autograd + ctypes costs tens of microseconds of host time
 // per forward+backward, more than the kernels of the small ops (q_nstep_td, PPO, C51).
 //
-// Argument order follows the `*Function.apply` of di_hpc_b200/rl_utils/*.py; nothing here computes.
+// Argument order follows the `*Function.apply` of di_hpc_b200/{rl_utils,torch_utils/network}/*.py; nothing here
+// computes.
 #include "common.h"
 
 namespace hpcrl {
@@ -407,6 +408,49 @@ struct IqnFn : public Function<IqnFn> {
     }
 };
 
+// ------------------------------------------------------------------------------------------------ ScatterConnection
+int scatter_mode(const std::string& scatter_type) {
+    TORCH_CHECK_VALUE(scatter_type == "cover" || scatter_type == "add", "scatter_type must be 'cover' or 'add', got '",
+                      scatter_type, "'");
+    return scatter_type == "add" ? HPC_RLL_SCATTER_ADD : HPC_RLL_SCATTER_COVER;
+}
+
+struct ScatterConnectionFn : public Function<ScatterConnectionFn> {
+    static Tensor forward(AutogradContext* ctx, const Tensor& x_, const Tensor& location_, int64_t H, int64_t W,
+                          const std::string& scatter_type) {
+        const Tensor x = f32(x_, "x"), location = i64(location_, "location");
+        TORCH_CHECK_VALUE(x.dim() == 3, "x must be (B, M, N), got ", x.sizes());
+        const int64_t B = x.size(0), M = x.size(1), N = x.size(2);
+        TORCH_CHECK_VALUE(location.dim() == 3 && location.size(0) == B && location.size(1) == M && location.size(2) == 2,
+                          "location must be (B, M, 2)=(", B, ", ", M, ", 2), got ", location.sizes());
+        TORCH_CHECK_VALUE(location.device() == x.device(), "x and location must be on one device");
+        TORCH_CHECK_VALUE(H >= 0 && W >= 0, "spatial size must be non-negative");
+        const int mode = scatter_mode(scatter_type);
+        c10::cuda::CUDAGuard guard(x.device());
+        Tensor out = torch::empty({B, N, H, W}, x.options());
+        ck(hpc_rll_scatter_connection_forward(fp(x), ip(location), fpm(out), B, M, N, H, W, mode, cur_stream()),
+           "hpc_rll_scatter_connection_forward");
+        ctx->save_for_backward({location});
+        ctx->saved_data["H"] = H;
+        ctx->saved_data["W"] = W;
+        return out;
+    }
+    static variable_list backward(AutogradContext* ctx, variable_list grads) {
+        const Tensor location = ctx->get_saved_variables()[0];
+        const int64_t B = location.size(0), M = location.size(1);
+        const int64_t H = ctx->saved_data["H"].toInt(), W = ctx->saved_data["W"].toInt();
+        const Tensor g = f32(grads[0], "grad_out");
+        TORCH_CHECK_VALUE(g.dim() == 4 && g.size(0) == B && g.size(2) == H && g.size(3) == W,
+                          "grad_out must be (B, N, H, W), got ", g.sizes());
+        const int64_t N = g.size(1);
+        c10::cuda::CUDAGuard guard(g.device());
+        Tensor gx = torch::empty({B, M, N}, g.options());
+        ck(hpc_rll_scatter_connection_backward(fp(g), ip(location), fpm(gx), B, M, N, H, W, cur_stream()),
+           "hpc_rll_scatter_connection_backward");
+        return {gx, Tensor(), Tensor(), Tensor(), Tensor()};
+    }
+};
+
 // ------------------------------------------------------------------------------------------------ P2P all-reduce
 // all-reduce(SUM) of <= 16 loss scalars over NVLink peer memory (csrc/p2p.cu); gradient = identity.  `bufs_addr` is the
 // address of the host array of `world` device pointers held by di_hpc_b200.sharding.P2PScalarAllReduce.
@@ -476,6 +520,11 @@ void register_fast_ops(pybind11::module& m) {
               return QrdqnFn::apply(q, nq, a, na, r, d, w, vg, g, gb);
           },
           "QR-DQN n-step TD error with autograd");
+    m.def("scatter_connection",
+          [](const Tensor& x, const Tensor& location, int64_t H, int64_t W, const std::string& scatter_type) {
+              return ScatterConnectionFn::apply(x, location, H, W, scatter_type);
+          },
+          "ScatterConnection (B,M,N) -> (B,N,H,W), 'cover' or 'add', with autograd (gather backward)");
     m.def("iqn_nstep_td",
           [](const Tensor& q, const Tensor& nq, const Tensor& a, const Tensor& na, const Tensor& r, const Tensor& d,
              const Tensor& rq, const OptTensor& w, const OptTensor& vg, double g, double k, int64_t gb) {

@@ -1,4 +1,5 @@
 // legacy.cpp -- the reference's native boundary: the 19 hot-path entry points of the pybind module `hpc_rl_utils`
+// and the two ScatterConnection entry points of `hpc_torch_utils_network` (in the submodule `_torch_utils_network`)
 // (/root/reference/src/rl_utils/entry.cpp:20-38, declared in include/hpc/rll/cuda/rl_utils/entry.h:62-165), with the
 // SAME names, the same `(inputs: List[Tensor], outputs: List[Tensor], float...)` shape and the same positional tensor
 // order as each reference launcher (src/rl_utils/*.cu, `index++` unpacking), implemented on top of the C ABI.
@@ -323,6 +324,39 @@ void PPOBackward(const TL& in, TL& out) {
        "hpc_rll_axpby");
 }
 
+// ---- scatter_connection (src/torch_utils/network/scatter_connection.cu) --------------------------------------------
+// inputs {x (B,M,N), location (B,M,2)}, outputs {out (B,N,H,W)}: H and W come from the caller's output tensor
+void ScatterConnectionForward(const TL& in, TL& out, const std::string& scatter_type) {
+    need(in, 2, "ScatterConnectionForward inputs");
+    need(out, 1, "ScatterConnectionForward outputs");
+    TORCH_CHECK(scatter_type == "cover" || scatter_type == "add", "scatter_type must be 'cover' or 'add'");
+    const Tensor x = f32(in[0], "input"), loc = i64(in[1], "location");
+    TORCH_CHECK(x.dim() == 3 && out[0].dim() == 4, "input must be (B, M, N) and output (B, N, H, W)");
+    const int64_t B = x.size(0), M = x.size(1), N = x.size(2), H = out[0].size(2), W = out[0].size(3);
+    TORCH_CHECK(out[0].size(0) == B && out[0].size(1) == N, "output must be (B, N, H, W)=(", B, ", ", N, ", H, W)");
+    TORCH_CHECK(loc.numel() == B * M * 2, "location must be (B, M, 2)");
+    c10::cuda::CUDAGuard guard(x.device());
+    ck(hpc_rll_scatter_connection_forward(fp(x), ip(loc), outp(out[0], "output", B * N * H * W), B, M, N, H, W,
+                                          scatter_type == "add" ? HPC_RLL_SCATTER_ADD : HPC_RLL_SCATTER_COVER,
+                                          cur_stream()),
+       "hpc_rll_scatter_connection_forward");
+}
+
+// inputs {grad_out (B,N,H,W), location (B,M,2)}, outputs {grad_in (B,M,N)}
+void ScatterConnectionBackward(const TL& in, TL& out) {
+    need(in, 2, "ScatterConnectionBackward inputs");
+    need(out, 1, "ScatterConnectionBackward outputs");
+    const Tensor g = f32(in[0], "grad_out"), loc = i64(in[1], "location");
+    TORCH_CHECK(g.dim() == 4 && out[0].dim() == 3, "grad_out must be (B, N, H, W) and grad_in (B, M, N)");
+    const int64_t B = out[0].size(0), M = out[0].size(1), N = out[0].size(2), H = g.size(2), W = g.size(3);
+    TORCH_CHECK(g.size(0) == B && g.size(1) == N, "grad_out must be (B, N, H, W)=(", B, ", ", N, ", H, W)");
+    TORCH_CHECK(loc.numel() == B * M * 2, "location must be (B, M, 2)");
+    c10::cuda::CUDAGuard guard(g.device());
+    ck(hpc_rll_scatter_connection_backward(fp(g), ip(loc), outp(out[0], "grad_in", B * M * N), B, M, N, H, W,
+                                           cur_stream()),
+       "hpc_rll_scatter_connection_backward");
+}
+
 }  // namespace
 
 void register_legacy(pybind11::module& m) {
@@ -345,6 +379,11 @@ void register_legacy(pybind11::module& m) {
     m.def("IQNNStepTDErrorBackward", &IQNNStepTDErrorBackward, "iqn_nstep_td_error backward (CUDA)");
     m.def("QRDQNNStepTDErrorForward", &QRDQNNStepTDErrorForward, "qrdqn_nstep_td_error forward (CUDA)");
     m.def("QRDQNNStepTDErrorBackward", &QRDQNNStepTDErrorBackward, "qrdqn_nstep_td_error backward (CUDA)");
+    // the reference's second native module, `hpc_torch_utils_network` (src/torch_utils/network/entry.cpp), as a
+    // submodule so that `hpc_rl_utils` keeps exactly its own names; LstmForward / LstmBackward are not provided
+    auto net = m.def_submodule("_torch_utils_network", "the reference's hpc_torch_utils_network binding names");
+    net.def("ScatterConnectionForward", &ScatterConnectionForward, "scatter_connection forward (CUDA)");
+    net.def("ScatterConnectionBackward", &ScatterConnectionBackward, "scatter_connection backward (CUDA)");
 }
 
 }  // namespace hpcrl

@@ -1,0 +1,1 @@
+"""Host-side mirror of the reference package `hpc_rll.torch_utils` (network.scatter_connection; the LSTM is not provided)."""

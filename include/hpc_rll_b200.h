@@ -301,6 +301,24 @@ int hpc_rll_oracle_split_group(const int64_t* shapes, int64_t n, int ndim, int g
 int hpc_rll_sample_split_group(const int64_t* shapes, int64_t n, int ndim, int group, uint64_t seed,
                                int64_t* starts, int* n_groups);
 
+/* ---- ScatterConnection (torch_utils.network) -------------------------------------------------------
+ * replaces ScatterConnectionForward / ScatterConnectionBackward (/root/reference/src/torch_utils/network/
+ * scatter_connection.cu, kernels include/hpc/rll/cuda/torch_utils/network/scatter_connection_kernel.h); semantics of
+ * hpc_rll/origin/scatter_connection.py.
+ *   forward : x (B,M,N), location (B,M,2) int64 (y, x) -> out (B,N,H,W).  Cells no entity lands on are 0; otherwise
+ *             COVER: the row of the entity with the largest m on the cell, ADD: the fp32 sum over the cell's entities
+ *             in increasing m starting from +0.0.  Every element of `out` is written exactly once (no memset first).
+ *   backward: grad_out (B,N,H,W) -> grad_x (B,M,N), grad_x[b,m,:] = grad_out[b,:,y_m,x_m] in both modes.
+ * An entity with y outside [0,H) or x outside [0,W) is dropped: it writes nothing and its gradient is 0.
+ * Deterministic (no atomics), no allocation, no synchronisation.  A pointer may be NULL only when its tensor is
+ * empty. */
+#define HPC_RLL_SCATTER_COVER 0
+#define HPC_RLL_SCATTER_ADD 1
+int hpc_rll_scatter_connection_forward(const float* x, const int64_t* location, float* out, int64_t B, int64_t M,
+                                       int64_t N, int64_t H, int64_t W, int mode, void* stream);
+int hpc_rll_scatter_connection_backward(const float* grad_out, const int64_t* location, float* grad_x, int64_t B,
+                                        int64_t M, int64_t N, int64_t H, int64_t W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
