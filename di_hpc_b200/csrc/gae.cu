@@ -17,7 +17,7 @@
 // plus the d_t slice are TMA-staged through a shared-memory ring; BT consumer threads own one
 // column each, carry (g, v_{t+1}) in registers and stream results out with evict-first stores.
 // From 256 columns per SM up the OUTPUT is TMA-staged as well (ScanPipeOut: results collected in shared-memory
-// boxes and written with cp.async.bulk.tensor stores; gae_*_tma_st, configs 30-34) -- the fastest backward at the
+// boxes and written with cp.async.bulk.tensor stores; gae_*_tma_st, config 33) -- the fastest backward at the
 // headline shape (see pick_cfg).
 // HBM traffic = algorithmic: fwd 12 B/step, bwd 12 B/step (+ one extra value row).
 //
@@ -656,26 +656,23 @@ static int launch_bwd_tma_st(const float* grad_adv, int64_t ldg, const float* dt
     return HPC_RLL_OK;
 }
 
-// configuration table (index = hpc_rll_debug_set_config(HPC_RLL_OP_GAE, i)); -1/auto picks by B.
-//   0: BT=64  TT=16 ST=3      1: BT=128 TT=16 ST=3     2: BT=32 TT=32 ST=3
-//   3: BT=64  TT=32 ST=3      4: BT=128 TT=8  ST=4     5: BT=64 TT=8  ST=6
-//   6: BT=128 TT=32 ST=3      7: BT=256 TT=8  ST=4     8: BT=256 TT=16 ST=3
-//  10: BT=256 TT=4  ST=8     11: BT=256 TT=8  ST=6     13: BT=32 TT=64 ST=6   14: BT=32 TT=16 ST=12
-//  21: single-launch T-split with look-back (automatic for B <= 2048, T >= 512; 20 = its old two-launch name)   99: generic (non-TMA) kernel
-//  30..34: TMA-staged OUTPUT as well (ScanPipeOut; results leave as (TT x BT) bulk stores):
-//  30: BT=256 TT=8 ST=4    31: BT=128 TT=16 ST=3    32: BT=256 TT=16 ST=3    33: BT=256 TT=4 ST=6    34: BT=256 TT=4 ST=5
-//  35: BT=64 TT=16 ST=4    36: BT=128 TT=8 ST=5     37: BT=64 TT=8 ST=6       38: BT=128 TT=4 ST=8   (mid-size batches)
-// (a TMA box dimension is limited to 256 elements, so BT <= 256)
-// forced values >= 100 encode different kernels per direction: forward = v % 100, backward = v / 100
-static int pick_cfg(int64_t B, bool backward = false) {
-    int forced = tuning_config(HPC_RLL_OP_GAE);
-    if (forced >= 100) forced = backward ? forced / 100 : forced % 100;
+// Kernel regimes; hpc_rll_debug_set_config(HPC_RLL_OP_GAE, id) forces one, -1 picks by B.  <BT,TT,ST> = columns per
+// CTA, rows per TMA box, ring stages (a TMA box dimension is limited to 256 elements, so BT <= 256).
+//   33 wide (B >= 256*SMs, all operands TMA-describable): fwd gae_fwd_tma_st<256,4,5>, bwd gae_bwd_tma_st<256,4,6>
+//    7 wide, an output not TMA-describable:               gae_fwd_tma / gae_bwd_tma <256,8,4>
+//    5 mid (32*SMs <= B < 256*SMs):                        gae_fwd_tma / gae_bwd_tma <64,8,6>
+//   13 narrow (B < 32*SMs):                                gae_fwd_tma / gae_bwd_tma <32,64,6>
+//   21 single-launch T-split with look-back (automatic for B <= 2048, T >= 512; see lookback_geometry)
+//   99 generic (non-TMA) kernels, used when an input is not TMA-describable
+// gae_forward_moments runs gae_fwd_tma<...,true> with <256,8,4> (33, 7), <64,16,3> (5), <32,64,6> (13).
+static int pick_cfg(int64_t B) {
+    const int forced = tuning_config(HPC_RLL_OP_GAE);
     if (forced >= 0) return forced;
     const int64_t sms = sm_count();
     // tools/tune_gae.py on H100 at T=1024, B=65536 (median of 20 single calls): the bulk-store output kernels with
     // shallow boxes give the fastest backward (0.295 ms against 0.300-0.31 for per-thread stores) and a forward within
     // 1 % of the fastest
-    if (B >= 256 * sms) return backward ? 33 : 34;
+    if (B >= 256 * sms) return 33;
     // mid-size batches, same sweep at B = 8192 ... 32768: <64,8,6> (a deep row pipeline on narrow tiles) is the
     // fastest or within 5 % of it everywhere, fwd+bwd 0.091 ms at B=8192 against 0.113 for <32,32,3> and 0.229 ms at
     // B=24576 against 0.238 for <128,16,3>
@@ -721,44 +718,23 @@ static int gae_forward_impl(const float* value, int64_t ldv, const float* reward
         return HPC_RLL_OK;
     }
     int cfg = pick_cfg(B);
-    if (cfg == 20 || cfg == 21) cfg = 13;
+    if (cfg == 21) cfg = 13;
     // the d_t slice of a stage is a 16-byte-aligned bulk copy: a chunk must start on an even row
     const bool tma = tma_ok_2d(value, B, ldv) && tma_ok_2d(reward, B, ldr) && aligned16(dtab);
     if (!tma) cfg = 99;
-    if (cfg >= 30 && cfg < 99 && !tma_ok_2d(adv, B, lda)) cfg = 7;  // output not TMA-describable: per-thread stores
+    if (cfg == 33 && !tma_ok_2d(adv, B, lda)) cfg = 7;  // output not TMA-describable: per-thread stores
 #define HPC_FWD(BT_, TT_, ST_) \
     return launch_fwd_tma<BT_, TT_, ST_>(value, ldv, reward, ldr, dtab, adv, lda, T, B, g, f, stream, nullptr, nullptr, \
                                          v_next, carry)
-#define HPC_FWD_ST(BT_, TT_, ST_) \
-    return launch_fwd_tma_st<BT_, TT_, ST_>(value, ldv, reward, ldr, dtab, adv, lda, T, B, g, f, stream, v_next, carry)
     switch (cfg) {
-        case 0: HPC_FWD(64, 16, 3);
-        case 1: HPC_FWD(128, 16, 3);
-        case 2: HPC_FWD(32, 32, 3);
-        case 3: HPC_FWD(64, 32, 3);
-        case 4: HPC_FWD(128, 8, 4);
         case 5: HPC_FWD(64, 8, 6);
-        case 6: HPC_FWD(128, 32, 3);
         case 7: HPC_FWD(256, 8, 4);
-        case 8: HPC_FWD(256, 16, 3);
-        case 10: HPC_FWD(256, 4, 8);
-        case 11: HPC_FWD(256, 8, 6);
         case 13: HPC_FWD(32, 64, 6);
-        case 14: HPC_FWD(32, 16, 12);
-        // 30..: TMA-staged output (needs a TMA-describable adv as well; checked above)
-        case 30: HPC_FWD_ST(256, 8, 4);
-        case 31: HPC_FWD_ST(128, 16, 3);
-        case 32: HPC_FWD_ST(256, 16, 3);
-        case 33: HPC_FWD_ST(256, 4, 6);
-        case 34: HPC_FWD_ST(256, 4, 5);
-        case 35: HPC_FWD_ST(64, 16, 4);
-        case 36: HPC_FWD_ST(128, 8, 5);
-        case 37: HPC_FWD_ST(64, 8, 6);
-        case 38: HPC_FWD_ST(128, 4, 8);
+        case 33:
+            return launch_fwd_tma_st<256, 4, 5>(value, ldv, reward, ldr, dtab, adv, lda, T, B, g, f, stream, v_next, carry);
         default: break;
     }
 #undef HPC_FWD
-#undef HPC_FWD_ST
     const unsigned grid = static_cast<unsigned>((B + 127) / 128);
     gae_fwd_generic<false><<<grid, 128, 0, stream>>>(value, ldv, reward, ldr, dtab, adv, lda, static_cast<int>(T),
                                                      static_cast<int>(B), g, f, nullptr, v_next, carry);
@@ -805,20 +781,14 @@ static int gae_forward_moments_impl(const float* value, const float* reward, flo
     int cfg = pick_cfg(B);
     if (!(tma_ok_2d(value, B, B) && tma_ok_2d(reward, B, B))) cfg = 99;
     int nblocks = 0;
-    switch (cfg) {  // the tile shapes the automatic choice uses; anything else maps to the nearest of them
-        case 7: case 8: case 10: case 11: case 30: case 32: case 33: case 34:
+    switch (cfg) {
+        case 7: case 33:
             rc = launch_fwd_tma<256, 8, 4, true>(value, B, reward, B, dtab, adv, B, T, B, g, f, stream, partials, &nblocks);
             break;
-        case 1: case 4: case 6: case 31: case 36: case 38:
-            rc = launch_fwd_tma<128, 16, 3, true>(value, B, reward, B, dtab, adv, B, T, B, g, f, stream, partials, &nblocks);
-            break;
-        case 0: case 3: case 5: case 35: case 37:
+        case 5:
             rc = launch_fwd_tma<64, 16, 3, true>(value, B, reward, B, dtab, adv, B, T, B, g, f, stream, partials, &nblocks);
             break;
-        case 2: case 14:
-            rc = launch_fwd_tma<32, 32, 3, true>(value, B, reward, B, dtab, adv, B, T, B, g, f, stream, partials, &nblocks);
-            break;
-        case 13: case 20:
+        case 13:
             rc = launch_fwd_tma<32, 64, 6, true>(value, B, reward, B, dtab, adv, B, T, B, g, f, stream, partials, &nblocks);
             break;
         default: {
@@ -872,42 +842,22 @@ static int gae_backward_impl(const float* grad_adv, int64_t ldg, float* gv, int6
         HPC_LAUNCH_CHECK();
         return HPC_RLL_OK;
     }
-    int cfg = pick_cfg(B, true);
-    if (cfg == 20 || cfg == 21) cfg = 13;
+    int cfg = pick_cfg(B);
+    if (cfg == 21) cfg = 13;
     if (!(tma_ok_2d(grad_adv, B, ldg) && aligned16(dtab))) cfg = 99;
-    if (cfg >= 30 && cfg < 99 && !(tma_ok_2d(gv, B, ldgv) && tma_ok_2d(gr, B, ldgr))) cfg = 7;
+    if (cfg == 33 && !(tma_ok_2d(gv, B, ldgv) && tma_ok_2d(gr, B, ldgr))) cfg = 7;
 #define HPC_BWD(BT_, TT_, ST_) \
     return launch_bwd_tma<BT_, TT_, ST_>(grad_adv, ldg, dtab, gv, ldgv, gr, ldgr, T, B, g, f, stream, carry, write_last)
-#define HPC_BWD_ST(BT_, TT_, ST_) \
-    return launch_bwd_tma_st<BT_, TT_, ST_>(grad_adv, ldg, dtab, gv, ldgv, gr, ldgr, T, B, g, f, stream, carry, write_last)
     switch (cfg) {
-        case 0: HPC_BWD(64, 16, 3);
-        case 1: HPC_BWD(128, 16, 3);
-        case 2: HPC_BWD(32, 32, 3);
-        case 3: HPC_BWD(64, 32, 3);
-        case 4: HPC_BWD(128, 8, 4);
         case 5: HPC_BWD(64, 8, 6);
-        case 6: HPC_BWD(128, 32, 3);
         case 7: HPC_BWD(256, 8, 4);
-        case 8: HPC_BWD(256, 16, 3);
-        case 10: HPC_BWD(256, 4, 8);
-        case 11: HPC_BWD(256, 8, 6);
         case 13: HPC_BWD(32, 64, 6);
-        case 14: HPC_BWD(32, 16, 12);
-        // 30..: TMA-staged output (needs TMA-describable grad_value / grad_reward as well; checked above)
-        case 30: HPC_BWD_ST(256, 8, 4);
-        case 31: HPC_BWD_ST(128, 16, 3);
-        case 32: HPC_BWD_ST(256, 16, 3);
-        case 33: HPC_BWD_ST(256, 4, 6);
-        case 34: HPC_BWD_ST(256, 4, 5);
-        case 35: HPC_BWD_ST(64, 16, 4);
-        case 36: HPC_BWD_ST(128, 8, 5);
-        case 37: HPC_BWD_ST(64, 8, 6);
-        case 38: HPC_BWD_ST(128, 4, 8);
+        case 33:
+            return launch_bwd_tma_st<256, 4, 6>(grad_adv, ldg, dtab, gv, ldgv, gr, ldgr, T, B, g, f, stream, carry,
+                                                write_last);
         default: break;
     }
 #undef HPC_BWD
-#undef HPC_BWD_ST
     const unsigned grid = static_cast<unsigned>((B + 127) / 128);
     gae_bwd_generic<<<grid, 128, 0, stream>>>(grad_adv, ldg, dtab, gv, ldgv, gr, ldgr, static_cast<int>(T),
                                               static_cast<int>(B), g, f, carry, write_last);

@@ -269,14 +269,12 @@ int hpc_rll_td_lambda_forward(const float* value, const float* reward, const flo
         switch (cfg) {
             case 0: rc = launch_tdl_tma<3, 64, 16, 3>(value, reward, weight, grad_buf, partials, T, B, g, disc, gmd, nin, stream, &nblocks); break;
             case 1: rc = launch_tdl_tma<3, 256, 8, 4>(value, reward, weight, grad_buf, partials, T, B, g, disc, gmd, nin, stream, &nblocks); break;
-            case 3: rc = launch_tdl_tma<3, 128, 16, 3>(value, reward, weight, grad_buf, partials, T, B, g, disc, gmd, nin, stream, &nblocks); break;
             default: rc = launch_tdl_tma<3, 32, 32, 3>(value, reward, weight, grad_buf, partials, T, B, g, disc, gmd, nin, stream, &nblocks); break;
         }
     } else {
         switch (cfg) {
             case 0: rc = launch_tdl_tma<2, 64, 16, 3>(value, reward, weight, grad_buf, partials, T, B, g, disc, gmd, nin, stream, &nblocks); break;
             case 1: rc = launch_tdl_tma<2, 256, 8, 4>(value, reward, weight, grad_buf, partials, T, B, g, disc, gmd, nin, stream, &nblocks); break;
-            case 3: rc = launch_tdl_tma<2, 128, 16, 3>(value, reward, weight, grad_buf, partials, T, B, g, disc, gmd, nin, stream, &nblocks); break;
             default: rc = launch_tdl_tma<2, 32, 32, 3>(value, reward, weight, grad_buf, partials, T, B, g, disc, gmd, nin, stream, &nblocks); break;
         }
     }

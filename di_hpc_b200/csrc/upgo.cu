@@ -349,8 +349,6 @@ int hpc_rll_upgo_forward(const float* target_output, const float* rhos, const in
         HPC_LAUNCH_CHECK();
     } else if (cfg == 0) {
         rc = launch_upgo_scan<64, 8, 4>(bootstrap_values, rewards, rhos, metric, coef, partials, T, B, nin, stream, &nblocks);
-    } else if (cfg == 1) {
-        rc = launch_upgo_scan<128, 8, 4>(bootstrap_values, rewards, rhos, metric, coef, partials, T, B, nin, stream, &nblocks);
     } else {
         rc = launch_upgo_scan<32, 16, 3>(bootstrap_values, rewards, rhos, metric, coef, partials, T, B, nin, stream, &nblocks);
     }

@@ -527,12 +527,6 @@ int hpc_rll_vtrace_forward(const float* target_output, const float* behaviour_ou
                                                        T, B, g, f, rc, cc, pc, in, stream, nblocks2)
                      : launch_vtrace_scan<4, 64, 8, 4>(value, reward, is_buf, logp_buf, weight, pg_coef, gv_buf, part2,
                                                        T, B, g, f, rc, cc, pc, in, stream, nblocks2);
-    } else if (cfg == 1) {
-        nblocks2 = static_cast<int>((B + 127) / 128);
-        rc2 = weight ? launch_vtrace_scan<5, 128, 8, 3>(value, reward, is_buf, logp_buf, weight, pg_coef, gv_buf,
-                                                        part2, T, B, g, f, rc, cc, pc, in, stream, nblocks2)
-                     : launch_vtrace_scan<4, 128, 8, 3>(value, reward, is_buf, logp_buf, weight, pg_coef, gv_buf,
-                                                        part2, T, B, g, f, rc, cc, pc, in, stream, nblocks2);
     } else {
         nblocks2 = static_cast<int>((B + 31) / 32);
         rc2 = weight ? launch_vtrace_scan<5, 32, 16, 3>(value, reward, is_buf, logp_buf, weight, pg_coef, gv_buf,

@@ -59,7 +59,7 @@ def test_gae_vs_oracle_bitexact(T, B):
     if not exact:  # the same shape through the column-scan kernel is bit-exact
         from di_hpc_b200 import _abi
         try:
-            _abi.set_config(0, 2)
+            _abi.set_config(0, 13)
             adv, gv, gr = _run(value, reward, gadv, 0.99, 0.97)
         finally:
             _abi.set_config(0, -1)
@@ -81,11 +81,13 @@ def test_gae_vs_golden(name):
     assert rel_err(gr, c.grad("reward", 64)) <= 1e-5
 
 
-@pytest.mark.parametrize("cfg", [0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 11, 13, 14, 21, 30, 31, 32, 33, 34, 99])
+@pytest.mark.parametrize("cfg", [5, 7, 13, 21, 33, 99])
 def test_gae_every_kernel_config(cfg):
-    """All tile configurations (and the non-TMA kernel) must give identical bits; 21 = T-split with look-back."""
+    """Every kernel regime (and the non-TMA kernel) must give identical bits; 21 = T-split with look-back.  The
+    moments forward (gae_with_adv_stats) runs its own kernel for each regime and is bit-exact for all of them."""
     need_cuda()
     from di_hpc_b200 import _abi
+    from di_hpc_b200.rl_utils.gae import gae_with_adv_stats
     g = rng(77 + cfg)
     T, B = 203, 1300
     value = g.standard_normal((T + 1, B), dtype=np.float32)
@@ -94,12 +96,16 @@ def test_gae_every_kernel_config(cfg):
     try:
         _abi.set_config(0, cfg)
         adv, gv, gr = _run(value, reward, gadv, 0.95, 0.9)
+        adv_m, _ = gae_with_adv_stats(dev(value), dev(reward), 0.95, 0.9)
+        adv_m = host(adv_m)
     finally:
         _abi.set_config(0, -1)
     ob = orc.gae_backward(gadv, 0.95, 0.9)
-    same(adv, orc.gae_forward(value, reward, 0.95, 0.9), cfg != 21)
+    want = orc.gae_forward(value, reward, 0.95, 0.9)
+    same(adv, want, cfg != 21)
     same(gv, ob["value"], cfg != 21)
     same(gr, ob["reward"], cfg != 21)
+    same(adv_m, want, True)
 
 
 def test_gae_strided_views():

@@ -87,7 +87,7 @@ def test_vtrace_vs_golden(name):
         close_grad(gv, c.grad("value", prec), "grad_value")
 
 
-@pytest.mark.parametrize("cfg", [0, 1, 2, 99])
+@pytest.mark.parametrize("cfg", [0, 2, 99])
 def test_vtrace_scan_configs(cfg):
     need_cuda()
     from di_hpc_b200 import _abi

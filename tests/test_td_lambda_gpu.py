@@ -52,7 +52,7 @@ def test_td_lambda_vs_golden(name):
     assert grad_err(gv, c.grad("value", 32)) <= TOL and grad_err(gv, c.grad("value", 64)) <= TOL
 
 
-@pytest.mark.parametrize("cfg", [0, 1, 2, 3, 21, 99])  # 21 = single-launch T-split with look-back
+@pytest.mark.parametrize("cfg", [0, 1, 2, 21, 99])  # 21 = single-launch T-split with look-back
 def test_td_lambda_configs_agree(cfg):
     need_cuda()
     from di_hpc_b200 import _abi

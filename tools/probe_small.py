@@ -1,5 +1,5 @@
 """Small-batch regime (the reference's own test shapes, T=1024 B=64 ...): device time of GAE forward+backward per kernel
-configuration -- column scan (2, 13) vs the single-launch T-split with look-back (21, the automatic choice for B <= 4096)
+configuration -- column scan (5, 13) vs the single-launch T-split with look-back (21, the automatic choice for B <= 4096)
 -- measured three ways: raw C-ABI calls between events, CUDA-graph replay of fwd+bwd (what a captured training step
 sees), and the module API (GAE.forward + autograd) per call.
 
@@ -30,7 +30,7 @@ def main():
         adv, gv, gr = torch.empty(T, B, device="cuda"), torch.empty(T + 1, B, device="cuda"), torch.empty(T, B, device="cuda")
         m = GAE(T, B)
         side = torch.cuda.Stream()
-        for cfg in (2, 13, 21, -1):
+        for cfg in (5, 13, 21, -1):
             _abi.set_config(0, cfg)
 
             def raw(st):

@@ -60,7 +60,7 @@ def main():
         torch.cuda.synchronize()
         res["zero_copy_bit_exact"] = bool(torch.equal(da.cpu(), ha) and torch.equal(dgv.cpu(), hgv)
                                           and torch.equal(dgr.cpu(), hgr))
-        for cfg in (7, 30, 32, 11, 8):
+        for cfg in (5, 7, 13, 33):
             _abi.set_config(0, cfg)
             res["zero_copy_both_ms_cfg%d" % cfg] = timeit(both, 3)
         _abi.set_config(0, -1)

@@ -24,11 +24,11 @@ def r(*s):
 
 
 def wide_and_fused():
-    """kernels added late in round 1: TMA-staged output (ScanPipeOut, configs 30-34 = the default for wide batches),
+    """kernels added late in round 1: TMA-staged output (ScanPipeOut, config 33 = the default for wide batches),
     GAE with moments + PPO with fused normalisation, 64-bit / staged row paths (N = 18 / 9)"""
     T, B = 7, 40000
     v, rew = r(T + 1, B).requires_grad_(True), r(T, B).requires_grad_(True)
-    for cfg in (-1, 30, 31, 32, 33, 34):
+    for cfg in (-1, 7, 33):
         _abi.set_config(0, cfg)
         torch.autograd.grad(GAE(T, B)(v, rew), [v, rew], grad_outputs=r(T, B))
     _abi.set_config(0, -1)
@@ -93,7 +93,7 @@ def main():
     small_batch_tsplit()
     for T, B, N in ((37, 132, 6), (16, 260, 16), (9, 64, 40)):
         v, rew = r(T + 1, B).requires_grad_(True), r(T, B).requires_grad_(True)
-        for cfg in (-1, 0, 2, 13, 21, 99):
+        for cfg in (-1, 5, 13, 21, 99):
             _abi.set_config(0, cfg)
             torch.autograd.grad(GAE(T, B)(v, rew), [v, rew], grad_outputs=r(T, B))
         _abi.set_config(0, -1)

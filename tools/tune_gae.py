@@ -1,4 +1,4 @@
-"""Sweep GAE kernel configurations on the GPU: per-config fwd / bwd time (CUDA events) and GB/s."""
+"""Time the GAE kernel regimes on the GPU (gae.cu:pick_cfg): per-regime fwd / bwd time (CUDA events) and GB/s."""
 import json
 import os
 import sys
@@ -26,7 +26,7 @@ def time_fn(fn, iters=20, warm=3):
 def main():
     T = int(os.environ.get("T", 1024))
     B = int(os.environ.get("B", 65536))
-    cfgs = [int(c) for c in os.environ.get("CFGS", "0,1,4,7,8,10,11,99").split(",")]
+    cfgs = [int(c) for c in os.environ.get("CFGS", "5,7,13,21,33,99").split(",")]
     L = _abi.lib()
     v = torch.randn(T + 1, B, device="cuda")
     r = torch.randn(T, B, device="cuda")
