@@ -71,6 +71,9 @@ void count_launch(int n = 1);
 bool tma_ok_2d(const void* base, int64_t cols, int64_t ld);
 int make_tmap_2d(CUtensorMap* out, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
                  int box_cols, bool swizzle128 = false);  // swizzle128: CU_TENSOR_MAP_SWIZZLE_128B (box_cols <= 32)
+// the same for a uint8 tensor (masks): base 16B aligned, ld % 16 == 0, box_cols % 16 == 0
+int make_tmap_2d_u8(CUtensorMap* out, const uint8_t* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
+                    int box_cols);
 
 // Opt a kernel into > 48 KB dynamic shared memory.  The attribute is per context and holds the LARGEST byte count
 // granted so far per device: kernels whose dynamic size varies at run time (n_atom / tau dependent, nstep.cu) are

@@ -40,7 +40,7 @@ int sm_count() {
 static void init_cfg() {
     static const char* names[HPC_RLL_OP_COUNT] = {"GAE", "TD_LAMBDA", "VTRACE", "UPGO", "PPO",
                                                   "Q_NSTEP_TD", "DIST_NSTEP_TD", "QRDQN_NSTEP_TD", "IQN_NSTEP_TD",
-                                                  "GAE_MOMENTS"};
+                                                  "GAE_MOMENTS", "GAE_EPISODIC"};
     for (int i = 0; i < HPC_RLL_OP_COUNT; ++i) {
         char key[64];
         snprintf(key, sizeof(key), "HPC_RLL_CFG_%s", names[i]);
@@ -91,6 +91,23 @@ int make_tmap_2d(CUtensorMap* out, const float* base, int64_t rows, int64_t cols
     if (r != CUDA_SUCCESS)
         return set_error(HPC_RLL_ECUDA, "cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld ld=%lld", (int)r,
                          (long long)rows, (long long)cols, (long long)ld);
+    return HPC_RLL_OK;
+}
+
+int make_tmap_2d_u8(CUtensorMap* out, const uint8_t* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
+                    int box_cols) {
+    EncodeTiledFn fn = encode_fn();
+    if (!fn) return set_error(HPC_RLL_ECUDA, "cuTensorMapEncodeTiled entry point unavailable");
+    cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+    cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld)};
+    cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(base), dims, strides, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS)
+        return set_error(HPC_RLL_ECUDA, "cuTensorMapEncodeTiled (uint8) failed (%d) rows=%lld cols=%lld ld=%lld",
+                         (int)r, (long long)rows, (long long)cols, (long long)ld);
     return HPC_RLL_OK;
 }
 

@@ -234,4 +234,119 @@ struct ScanPipeOut {
     }
 };
 
+// ScanPipeMix -- ScanPipeOut with byte-wide inputs next to the fp32 ones (episode masks) and no row table.
+// maps.m[0..NF) are fp32 (TT x BT) boxes, maps.m[NF..NF+NB) uint8 (TT x BT) boxes (a byte box of a multiple of 32
+// columns and 4 rows is a multiple of 128 bytes, so every box of a stage stays 128-byte aligned).  Outputs are fp32
+// and TMA-stored as in ScanPipeOut.
+//   body.step(t, x, m, o): x[k] = fp32 input k, m[k] = byte input k at (t, col0+c); o[k] = output k
+template <int NF, int NB, int NOUT, int BT, int TT, int ST>
+struct ScanPipeMix {
+    static_assert(BT % 32 == 0, "column tile must be whole warps");
+    static_assert(TT % 4 == 0, "byte boxes must stay 128-byte aligned");
+    static constexpr int kConsumerWarps = BT / 32;
+    static constexpr int kThreads = BT + 32;  // + one producer warp
+    static constexpr int kBoxBytes = TT * BT * 4;
+    static constexpr int kByteBoxBytes = TT * BT;
+    static constexpr int kStageBytes = NF * kBoxBytes + NB * kByteBoxBytes;
+    static constexpr uint32_t kTxBytes = kStageBytes;
+    static constexpr int kNB = NB > 0 ? NB : 1;
+    static constexpr int kOutBytes = 2 * NOUT * kBoxBytes;  // two buffers per output
+    static constexpr int kSmemBytes = ST * kStageBytes + kOutBytes + 2 * ST * 8;
+
+    template <bool REVERSE, class Body>
+    static __device__ __forceinline__ void run(const TmapPack<NF + NB>& maps, const TmapPack<NOUT>& omaps, int T,
+                                               int col0, Body& body) {
+        extern __shared__ __align__(1024) unsigned char smem[];
+        float* obuf = reinterpret_cast<float*>(smem + ST * kStageBytes);
+        uint64_t* full = reinterpret_cast<uint64_t*>(smem + ST * kStageBytes + kOutBytes);
+        uint64_t* empty = full + ST;
+
+        const int tid = threadIdx.x;
+        const int nT = (T + TT - 1) / TT;
+        if (tid == 0) {
+#pragma unroll
+            for (int s = 0; s < ST; ++s) {
+                mbar_init(&full[s], 1);
+                mbar_init(&empty[s], kConsumerWarps);
+            }
+            fence_mbar_init();
+        }
+        __syncthreads();
+
+        if (tid >= BT) {
+            if (tid == BT) {
+#pragma unroll
+                for (int k = 0; k < NF + NB; ++k) prefetch_tmap(&maps.m[k]);
+                for (int it = 0; it < nT; ++it) {
+                    const int s = it % ST;
+                    if (it >= ST) mbar_wait(&empty[s], ((it / ST) & 1) ^ 1);
+                    const int j = REVERSE ? nT - 1 - it : it;
+                    unsigned char* st = smem + s * kStageBytes;
+                    mbar_arrive_expect_tx(&full[s], kTxBytes);
+#pragma unroll
+                    for (int k = 0; k < NF; ++k) tma_load_2d(st + k * kBoxBytes, &maps.m[k], col0, j * TT, &full[s]);
+#pragma unroll
+                    for (int k = 0; k < NB; ++k)
+                        tma_load_2d(st + NF * kBoxBytes + k * kByteBoxBytes, &maps.m[NF + k], col0, j * TT, &full[s]);
+                }
+            }
+            return;
+        }
+
+        const int c = tid;
+        if (tid == 0) {
+#pragma unroll
+            for (int k = 0; k < NOUT; ++k) prefetch_tmap(&omaps.m[k]);
+        }
+        for (int it = 0; it < nT; ++it) {
+            const int s = it % ST;
+            const int j = REVERSE ? nT - 1 - it : it;
+            const float* st = reinterpret_cast<const float*>(smem + s * kStageBytes);
+            const unsigned char* sb = smem + s * kStageBytes + NF * kBoxBytes;
+            float* ob = obuf + (it & 1) * (NOUT * TT * BT);
+            mbar_wait(&full[s], (it / ST) & 1);
+            const int rows = min(TT, T - j * TT);
+            if (rows == TT) {
+#pragma unroll
+                for (int ii = 0; ii < TT; ++ii) {
+                    const int i = REVERSE ? TT - 1 - ii : ii;
+                    float x[NF], o[NOUT];
+                    unsigned m[kNB];
+#pragma unroll
+                    for (int k = 0; k < NF; ++k) x[k] = st[(k * TT + i) * BT + c];
+#pragma unroll
+                    for (int k = 0; k < NB; ++k) m[k] = sb[(k * TT + i) * BT + c];
+                    body.step(j * TT + i, x, m, o);
+#pragma unroll
+                    for (int k = 0; k < NOUT; ++k) ob[(k * TT + i) * BT + c] = o[k];
+                }
+            } else {
+                for (int ii = 0; ii < rows; ++ii) {
+                    const int i = REVERSE ? rows - 1 - ii : ii;
+                    float x[NF], o[NOUT];
+                    unsigned m[kNB];
+#pragma unroll
+                    for (int k = 0; k < NF; ++k) x[k] = st[(k * TT + i) * BT + c];
+#pragma unroll
+                    for (int k = 0; k < NB; ++k) m[k] = sb[(k * TT + i) * BT + c];
+                    body.step(j * TT + i, x, m, o);
+#pragma unroll
+                    for (int k = 0; k < NOUT; ++k) ob[(k * TT + i) * BT + c] = o[k];
+                }
+            }
+            __syncwarp();
+            if ((tid & 31) == 0) mbar_arrive(&empty[s]);
+            fence_proxy_async_smem();
+            if (tid == 0) bulk_wait_group_read<0>();
+            named_bar_sync(1, BT);
+            if (tid == 0) {
+#pragma unroll
+                for (int k = 0; k < NOUT; ++k) tma_store_2d(&omaps.m[k], col0, j * TT, ob + k * TT * BT);
+                bulk_commit_group();
+            }
+        }
+        if (tid == 0) bulk_wait_group<0>();
+    }
+};
+
 }  // namespace hpcrll

@@ -49,6 +49,62 @@ struct GaeFn : public Function<GaeFn> {
     }
 };
 
+// ------------------------------------------------------------------------------------------------ episodic GAE
+// done / traj_flag as (T,B) bytes read in place: bool is viewed as uint8, uint8 is kept, any other dtype becomes
+// `mask != 0` (so a fractional float mask counts as set; DESIGN.md §7)
+inline Tensor mask_u8(const OptTensor& m_, const char* name, const Tensor& like) {
+    if (!m_.has_value() || !m_->defined()) return Tensor();
+    const Tensor& m = *m_;
+    TORCH_CHECK(m.is_cuda(), name, " must be a CUDA tensor (hpc version only supports cuda)");
+    TORCH_CHECK_VALUE(m.device() == like.device(), name, " must be on the device of reward");
+    TORCH_CHECK_VALUE(m.sizes() == like.sizes(), name, " must be (T, B)=", like.sizes(), ", got ", m.sizes());
+    if (m.scalar_type() == torch::kUInt8) return m.contiguous();
+    if (m.scalar_type() == torch::kBool) return m.contiguous().view(torch::kUInt8);
+    return m.ne(0).view(torch::kUInt8);
+}
+inline const uint8_t* u8p(const Tensor& t) { return t.defined() ? t.data_ptr<uint8_t>() : nullptr; }
+
+struct GaeEpisodicFn : public Function<GaeEpisodicFn> {
+    static Tensor forward(AutogradContext* ctx, const Tensor& value_, const Tensor& next_value_, const Tensor& reward_,
+                          const OptTensor& done_, const OptTensor& traj_, double gamma, double lambda) {
+        const Tensor value = f32(value_, "value"), next_value = f32(next_value_, "next_value");
+        const Tensor reward = f32(reward_, "reward");
+        TORCH_CHECK_VALUE(reward.dim() == 2, "reward must be (T, B), got ", reward.sizes());
+        TORCH_CHECK_VALUE(value.sizes() == reward.sizes() && next_value.sizes() == reward.sizes(),
+                          "value, next_value and reward must all be (T, B)=", reward.sizes(), ", got ", value.sizes(),
+                          " and ", next_value.sizes());
+        TORCH_CHECK_VALUE(value.device() == reward.device() && next_value.device() == reward.device(),
+                          "value, next_value and reward must be on one device");
+        const Tensor done = mask_u8(done_, "done", reward);
+        Tensor traj = mask_u8(traj_, "traj_flag", reward);
+        if (!traj.defined()) traj = done;  // traj_flag=None: episodes are cut where they end
+        const int64_t T = reward.size(0), B = reward.size(1);
+        c10::cuda::CUDAGuard guard(reward.device());
+        Tensor adv = torch::empty_like(reward);
+        ck(hpc_rll_gae_episodic_forward(fp(value), fp(next_value), fp(reward), u8p(done), u8p(traj), fpm(adv), T, B,
+                                        gamma, lambda, cur_stream()),
+           "hpc_rll_gae_episodic_forward");
+        ctx->save_for_backward({done, traj});
+        ctx->saved_data["gamma"] = gamma;
+        ctx->saved_data["lambda"] = lambda;
+        return adv;
+    }
+    static variable_list backward(AutogradContext* ctx, variable_list grads) {
+        const auto sv = ctx->get_saved_variables();
+        const Tensor &done = sv[0], &traj = sv[1];
+        const Tensor g = f32(grads[0], "grad_adv");
+        const int64_t T = g.size(0), B = g.size(1);
+        c10::cuda::CUDAGuard guard(g.device());
+        // one pass writes all three gradients; autograd drops the ones no input asked for
+        Tensor gv = torch::empty_like(g), gnv = torch::empty_like(g), gr = torch::empty_like(g);
+        ck(hpc_rll_gae_episodic_backward(fp(g), u8p(done), u8p(traj), fpm(gv), fpm(gnv), fpm(gr), T, B,
+                                         ctx->saved_data["gamma"].toDouble(), ctx->saved_data["lambda"].toDouble(),
+                                         cur_stream()),
+           "hpc_rll_gae_episodic_backward");
+        return {gv, gnv, gr, Tensor(), Tensor(), Tensor(), Tensor()};
+    }
+};
+
 // ------------------------------------------------------------------------------------------------ TD(lambda)
 struct TdLambdaFn : public Function<TdLambdaFn> {
     static Tensor forward(AutogradContext* ctx, const Tensor& value_, const Tensor& reward_, const OptTensor& weight_,
@@ -481,6 +537,10 @@ void register_fast_ops(pybind11::module& m) {
     namespace py = pybind11;
     m.def("gae", [](const Tensor& v, const Tensor& r, double g, double l) { return GaeFn::apply(v, r, g, l); },
           "GAE forward with autograd (adjoint)");
+    m.def("gae_episodic",
+          [](const Tensor& v, const Tensor& nv, const Tensor& r, const OptTensor& done, const OptTensor& traj, double g,
+             double l) { return GaeEpisodicFn::apply(v, nv, r, done, traj, g, l); },
+          "episode-aware (un-normalised) GAE with done / traj_flag masks, with autograd (adjoint)");
     m.def("td_lambda",
           [](const Tensor& v, const Tensor& r, const OptTensor& w, double g, double l, int64_t gb) {
               return TdLambdaFn::apply(v, r, w, g, l, gb);

@@ -7,15 +7,58 @@ reference (gae.py:20-61).  Differences, all deliberate (DESIGN.md "Deviations"):
   * the result is a fresh tensor sized from the inputs, not the module-owned ``adv`` buffer returned
     by alias (gae.py:39,61) -- T and B of the constructor are kept only for API compatibility;
   * kernels run on PyTorch's current stream, with argument checks.
+
+``gae(gae_data(value, next_value, reward, done, traj_flag))`` is the episode-aware, un-normalised GAE of DI-engine's
+functional ``ding.rl_utils.gae``, for rollouts whose columns hold several episodes.  The reference has no counterpart.
 """
+from collections import namedtuple
+
 import torch
 
 from .. import _abi, _ext
+
+gae_data = namedtuple('gae_data', ['value', 'next_value', 'reward', 'done', 'traj_flag'])
 
 
 @_ext.reference_function
 def GAEFunction(value, reward, gamma, lambda_):
     return _ext.require().gae(value, reward, float(gamma), float(lambda_))
+
+
+def gae(data, gamma: float = 0.99, lambda_: float = 0.97) -> torch.Tensor:
+    """
+    Overview:
+        Standard (un-normalised) Generalized Advantage Estimation over a ``(T, B)`` rollout segment in which episodes
+        may end anywhere, as DI-engine's ``ding.rl_utils.gae``.  This is NOT the normalised variant that ``GAE``
+        computes (no ``denom``).  With ``g = float32(gamma)`` and ``gl = float32(gamma * lambda_)``::
+
+            delta_t = (reward_t + g * next_value_t * (1 - done_t)) - value_t
+            adv_t   = delta_t + gl * (1 - traj_flag_t) * adv_{t+1},    adv_{T-1} = delta_{T-1}
+
+        Every step is one rounded fp32 operation in this order, so the result (and its gradients) match eager
+        PyTorch of the formula bit for bit; segments of long, narrow batches (B <= 2048, T >= 512) are scanned in
+        parallel pieces and agree to ~1e-7 relative instead.  Differentiable in ``value``, ``next_value`` and
+        ``reward``.
+    Arguments:
+        - data (:obj:`gae_data` or any 5-tuple): ``(value, next_value, reward, done, traj_flag)``
+            - value, next_value, reward (:obj:`torch.FloatTensor`): :math:`(T, B)`, ``next_value_t`` is the value of
+              the state after step t (the bootstrap value at an episode's end)
+            - done (:obj:`torch.Tensor` or None): :math:`(T, B)`; a set entry masks the bootstrap of that step.
+              None: no step ends an episode.
+            - traj_flag (:obj:`torch.Tensor` or None): :math:`(T, B)`; a set entry cuts the recursion after that step.
+              None: ``traj_flag = done``.
+            Masks may be bool or uint8 (read in place, non-zero = set); any other dtype is converted with
+            ``mask != 0``, so a fractional float mask counts as set.
+        - gamma (:obj:`float`): discount factor, defaults to 0.99
+        - lambda_ (:obj:`float`): GAE lambda, defaults to 0.97
+    Returns:
+        - adv (:obj:`torch.FloatTensor`): :math:`(T, B)`
+    """
+    value, next_value, reward, done, traj_flag = data
+    if value.dim() != 2:
+        raise ValueError("gae: value must be (T, B), got %s; multi-agent (T, B, A) values are not supported"
+                         % (tuple(value.shape), ))
+    return _ext.require().gae_episodic(value, next_value, reward, done, traj_flag, float(gamma), float(lambda_))
 
 
 def gae_with_adv_stats(value, reward, gamma: float = 0.99, lambda_: float = 0.97, group=None):

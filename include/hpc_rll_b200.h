@@ -47,7 +47,8 @@ extern "C" {
 #define HPC_RLL_OP_QRDQN_NSTEP_TD 7
 #define HPC_RLL_OP_IQN_NSTEP_TD 8
 #define HPC_RLL_OP_GAE_MOMENTS 9 /* workspace sizing only; tuning follows HPC_RLL_OP_GAE */
-#define HPC_RLL_OP_COUNT 10
+#define HPC_RLL_OP_GAE_EPISODIC 10
+#define HPC_RLL_OP_COUNT 11
 
 /* ---- library ------------------------------------------------------------------------------ */
 const char* hpc_rll_version(void);
@@ -122,6 +123,24 @@ int hpc_rll_gae_backward_chunk(const float* grad_adv, float* grad_value, float* 
 int hpc_rll_gae_fwd_bwd_host(const float* h_value, const float* h_reward, const float* h_grad_adv, float* h_adv,
                              float* h_grad_value, float* h_grad_reward, int64_t T, int64_t B, double gamma,
                              double lambda);
+
+/* ---- episode-aware GAE ------------------------------------------------------------------------
+ * Standard (un-normalised) GAE over a (T,B) segment that may hold several episodes per column, with DI-engine's
+ * gae_data(value, next_value, reward, done, traj_flag) inputs.  The reference has no counterpart.
+ *   value, next_value, reward (T,B) fp32; done_u8, traj_u8 (T,B) bytes, non-zero = set, NULL = all zero
+ *     delta_t = (reward_t + gamma * next_value_t * (1 - done_t)) - value_t
+ *     adv_t   = delta_t + gamma*lambda * (1 - traj_t) * adv_{t+1},   adv_{T-1} = delta_{T-1}
+ *   (gamma*lambda is formed in double and rounded once; every other step is one rounded fp32 operation)
+ * backward: grad_adv (T,B) -> grad_value, grad_next_value, grad_reward (T,B), all three written:
+ *     u_t = grad_adv_t + gamma*lambda*(1 - traj_{t-1}) * u_{t-1},  u_0 = grad_adv_0
+ *     grad_reward = u, grad_value = -u, grad_next_value = (gamma * u) * (1 - done)
+ * All tensors contiguous.  A data pointer may be NULL only when T*B == 0. */
+int hpc_rll_gae_episodic_forward(const float* value, const float* next_value, const float* reward,
+                                 const uint8_t* done_u8, const uint8_t* traj_u8, float* adv, int64_t T, int64_t B,
+                                 double gamma, double lambda, void* stream);
+int hpc_rll_gae_episodic_backward(const float* grad_adv, const uint8_t* done_u8, const uint8_t* traj_u8,
+                                  float* grad_value, float* grad_next_value, float* grad_reward, int64_t T, int64_t B,
+                                  double gamma, double lambda, void* stream);
 
 /* test hook: the stage heights hpc_rll_gae_fwd_bwd_host would use for a (T,B) problem (host-only, no CUDA call);
  * writes up to `cap` entries, returns the number of stages */
