@@ -258,7 +258,7 @@ __global__ void __launch_bounds__(256) ppo_rows_fwd_loop(const float* __restrict
         const float lsn = logf(sn), lso = logf(so);
         float h = 0.f;
         for (int k = lane; k < N; k += 32) {
-            const float lp = row_logp<true>(xn[k], mn, lsn);
+            const float lp = fmaxf(row_logp<true>(xn[k], mn, lsn), kNegBig);  // -inf logits: 0 * -3e38, not NaN
             h += exp_term(lp) * lp;
         }
         const float H = -warp_sum(h);

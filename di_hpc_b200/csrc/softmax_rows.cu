@@ -141,7 +141,7 @@ __global__ void __launch_bounds__(256) softmax_grad_rows_loop_kernel(const float
         if (ENT) {
             float h = 0.f;
             for (int k = lane; k < N; k += 32) {
-                const float l = row_logp<CAT>(x[k], m, logs);
+                const float l = fmaxf(row_logp<CAT>(x[k], m, logs), kNegBig);  // -inf logits: 0 * -3e38, not NaN
                 h += exp_term(l) * l;
             }
             H = -warp_sum(h);
@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(256) softmax_grad_rows_loop_kernel(const float
         const float c = s1 * c1[row];
         const float e2 = ENT ? s2 * (w ? w[row] : 1.f) : 0.f;
         for (int k = lane; k < N; k += 32) {
-            const float l = row_logp<CAT>(x[k], m, logs);
+            const float l = fmaxf(row_logp<CAT>(x[k], m, logs), kNegBig);  // p = 0 and a finite l for -inf logits
             const float p = exp_term(l);
             float gq = c * ((k == a ? 1.f : 0.f) - p);
             if (ENT) gq += e2 * (-p * (l + H));

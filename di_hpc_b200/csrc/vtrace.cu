@@ -166,7 +166,7 @@ __global__ void __launch_bounds__(256) vtrace_rows_fwd_loop(const float* __restr
         const float lst = logf(st), lsb = logf(sb);
         float h = 0.f;
         for (int k = lane; k < N; k += 32) {
-            const float lp = row_logp<true>(xt[k], mt, lst);
+            const float lp = fmaxf(row_logp<true>(xt[k], mt, lst), kNegBig);  // -inf logits: 0 * -3e38, not NaN
             h += exp_term(lp) * lp;
         }
         const float H = -warp_sum(h);
