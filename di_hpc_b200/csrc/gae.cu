@@ -16,7 +16,7 @@
 // Design: ScanPipe (scan_pipe.cuh) -- (TT x BT) boxes of value/reward (fwd) or grad_adv (bwd)
 // plus the d_t slice are TMA-staged through a shared-memory ring; BT consumer threads own one
 // column each, carry (g, v_{t+1}) in registers and stream results out with evict-first stores.
-// From 256 columns per SM up the OUTPUT is TMA-staged as well (ScanPipeOut: results collected in shared-memory
+// From 256 columns per SM up the OUTPUT is TMA-staged as well (NOUT > 0: results collected in shared-memory
 // boxes and written with cp.async.bulk.tensor stores; gae_*_tma_st, config 33) -- the fastest backward at the
 // headline shape (see pick_cfg).
 // HBM traffic = algorithmic: fwd 12 B/step, bwd 12 B/step (+ one extra value row).
@@ -136,6 +136,33 @@ __device__ __forceinline__ float div_by_table(float x, float d, float r) {
     return __fmaf_rn(__fmaf_rn(-d, q0, x), r, q0);
 }
 
+namespace {
+
+// one forward step: x = (v_t, r_t), dt = (d_t, 1/d_t), v1 = v_{t+1}; `g` = g_{t+1} on entry, g_t on exit.
+// Returns adv_t.
+__device__ __forceinline__ float fwd_step(const float (&x)[2], const float (&dt)[2], float v1, float gamma,
+                                          float factor, float& g) {
+    const float delta = __fsub_rn(__fadd_rn(x[1], __fmul_rn(gamma, v1)), x[0]);
+    g = __fadd_rn(__fmul_rn(dt[0], delta), __fmul_rn(factor, g));
+    return div_by_table(g, dt[0], dt[1]);
+}
+
+// one backward step: G = grad_adv_t, dt = (d_t, 1/d_t); `gh` = ghat_{t-1} on entry, ghat_t on exit; `prev` =
+// dd_{t-1} on entry, dd_t on exit.  Returns (grad_value_t, grad_reward_t) = (gamma*dd_{t-1} - dd_t, dd_t).
+struct BwdOut {
+    float gv, gr;
+};
+__device__ __forceinline__ BwdOut bwd_step(float G, const float (&dt)[2], float gamma, float factor, float& gh,
+                                           float& prev) {
+    gh = __fadd_rn(div_by_table(G, dt[0], dt[1]), __fmul_rn(factor, gh));
+    const float dd = __fmul_rn(dt[0], gh);
+    const BwdOut o{__fsub_rn(__fmul_rn(gamma, prev), dd), dd};
+    prev = dd;
+    return o;
+}
+
+}  // namespace
+
 // MOM: also accumulate sum(adv) and sum(adv^2) in fp64 (hpc_rll_gae_forward_moments)
 template <bool MOM = false>
 struct GaeFwdBody {
@@ -146,10 +173,7 @@ struct GaeFwdBody {
     double m1, m2;
     float p1, p2;  // fp32 partial moments of the current 16-row run, folded into m1/m2 at t % 16 == 0
     __device__ __forceinline__ void step(int t, const float (&x)[2], const float (&dt)[2]) {
-        // x[0] = v_t, x[1] = r_t, dt = (d_t, 1/d_t)
-        const float delta = __fsub_rn(__fadd_rn(x[1], __fmul_rn(gamma, v1)), x[0]);
-        g = __fadd_rn(__fmul_rn(dt[0], delta), __fmul_rn(factor, g));
-        const float a = div_by_table(g, dt[0], dt[1]);
+        const float a = fwd_step(x, dt, v1, gamma, factor, g);
         if (valid) st_stream(adv, a);
         if (MOM) {  // t descends to 0, so the last run is always flushed
             p1 += a;
@@ -188,7 +212,7 @@ __global__ void __launch_bounds__(BT + 32) gae_fwd_tma(const __grid_constant__ T
                                                         float gamma, float factor, double* __restrict__ partials) {
     // v_next: the value row that follows the last row of this launch (value[T], or the carried row of a T-chunk);
     // carry (nullable): (2,B) scan state of a T-chunked run -- g in/out, value row out (see gae_forward_chunk)
-    using Pipe = ScanPipe<2, BT, TT, ST, 2>;
+    using Pipe = ScanPipe<2, 0, 0, BT, TT, ST, 2>;
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
     GaeFwdBody<MOM> body;
@@ -204,7 +228,7 @@ __global__ void __launch_bounds__(BT + 32) gae_fwd_tma(const __grid_constant__ T
     body.adv = adv + static_cast<int64_t>(T - 1) * ld_adv + col;
     body.v1 = body.valid ? v_next[col] : 0.f;
     if (carry != nullptr && body.valid) body.g = carry[col];
-    Pipe::template run<true>(maps, dtab, T, col0, body);
+    Pipe::template run<true>(maps, {}, dtab, T, col0, body);
     if (carry != nullptr && body.valid) {
         carry[col] = body.g;
         carry[B + col] = body.v1;
@@ -223,16 +247,13 @@ struct GaeBwdBody {
     bool valid;
     // gv / gr are running pointers (&grad[t][col] of the next step; t ascending)
     __device__ __forceinline__ void step(int /*t*/, const float (&x)[1], const float (&dt)[2]) {
-        const float h = __fadd_rn(div_by_table(x[0], dt[0], dt[1]), __fmul_rn(factor, gh));
-        gh = h;
-        const float dd = __fmul_rn(dt[0], h);
+        const BwdOut o = bwd_step(x[0], dt, gamma, factor, gh, prev);
         if (valid) {
-            st_stream(gr, dd);
-            st_stream(gv, __fsub_rn(__fmul_rn(gamma, prev), dd));
+            st_stream(gr, o.gr);
+            st_stream(gv, o.gv);
         }
         gr += ld_gr;
         gv += ld_gv;
-        prev = dd;
     }
 };
 
@@ -245,7 +266,7 @@ __global__ void __launch_bounds__(BT + 32) gae_bwd_tma(const __grid_constant__ T
                                                         int write_last) {
     // carry (nullable): (2,B) = (ghat, dd of the previous row) of a T-chunked run; write_last: this launch ends at the
     // global row T-1, so row T of grad_value (= gamma*dd_{T-1}) is written as well
-    using Pipe = ScanPipe<1, BT, TT, ST, 2>;
+    using Pipe = ScanPipe<1, 0, 0, BT, TT, ST, 2>;
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
     GaeBwdBody body;
@@ -262,7 +283,7 @@ __global__ void __launch_bounds__(BT + 32) gae_bwd_tma(const __grid_constant__ T
         body.gh = carry[col];
         body.prev = carry[B + col];
     }
-    Pipe::template run<false>(maps, dtab, T, col0, body);
+    Pipe::template run<false>(maps, {}, dtab, T, col0, body);
     if (body.valid && write_last) st_stream(body.gv, __fmul_rn(gamma, body.prev));  // row T
     if (carry != nullptr && body.valid) {
         carry[col] = body.gh;
@@ -270,13 +291,12 @@ __global__ void __launch_bounds__(BT + 32) gae_bwd_tma(const __grid_constant__ T
     }
 }
 
-// ---- variants with TMA-staged OUTPUT (ScanPipeOut): same arithmetic, results leave as (TT x BT) bulk stores ----
+// ---- variants with TMA-staged OUTPUT (NOUT > 0): same arithmetic, results leave as (TT x BT) bulk stores ----
 struct GaeFwdBodyO {
     float g, v1, gamma, factor;
-    __device__ __forceinline__ void step(int /*t*/, const float (&x)[2], const float (&dt)[2], float (&o)[1]) {
-        const float delta = __fsub_rn(__fadd_rn(x[1], __fmul_rn(gamma, v1)), x[0]);
-        g = __fadd_rn(__fmul_rn(dt[0], delta), __fmul_rn(factor, g));
-        o[0] = div_by_table(g, dt[0], dt[1]);
+    __device__ __forceinline__ void step(int /*t*/, const float (&x)[2], const float (&dt)[2],
+                                         const unsigned (&)[1], float (&o)[1]) {
+        o[0] = fwd_step(x, dt, v1, gamma, factor, g);
         v1 = x[0];
     }
 };
@@ -288,7 +308,7 @@ __global__ void __launch_bounds__(BT + 32) gae_fwd_tma_st(const __grid_constant_
                                                            const float* __restrict__ v_next,
                                                            float* __restrict__ carry, int T, int B, float gamma,
                                                            float factor) {
-    using Pipe = ScanPipeOut<2, 1, BT, TT, ST, 2>;
+    using Pipe = ScanPipe<2, 0, 1, BT, TT, ST, 2>;
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
     const bool valid = threadIdx.x < BT && col < B;
@@ -306,13 +326,11 @@ __global__ void __launch_bounds__(BT + 32) gae_fwd_tma_st(const __grid_constant_
 
 struct GaeBwdBodyO {
     float gh, prev, gamma, factor;
-    __device__ __forceinline__ void step(int /*t*/, const float (&x)[1], const float (&dt)[2], float (&o)[2]) {
-        const float h = __fadd_rn(div_by_table(x[0], dt[0], dt[1]), __fmul_rn(factor, gh));
-        gh = h;
-        const float dd = __fmul_rn(dt[0], h);
-        o[0] = __fsub_rn(__fmul_rn(gamma, prev), dd);  // grad_value[t]
-        o[1] = dd;                                      // grad_reward[t]
-        prev = dd;
+    __device__ __forceinline__ void step(int /*t*/, const float (&x)[1], const float (&dt)[2],
+                                         const unsigned (&)[1], float (&o)[2]) {
+        const BwdOut r = bwd_step(x[0], dt, gamma, factor, gh, prev);
+        o[0] = r.gv;
+        o[1] = r.gr;
     }
 };
 
@@ -323,7 +341,7 @@ __global__ void __launch_bounds__(BT + 32) gae_bwd_tma_st(const __grid_constant_
                                                            float* __restrict__ grad_value, int64_t ld_gv, int T, int B,
                                                            float gamma, float factor, float* __restrict__ carry,
                                                            int write_last) {
-    using Pipe = ScanPipeOut<1, 2, BT, TT, ST, 2>;
+    using Pipe = ScanPipe<1, 0, 2, BT, TT, ST, 2>;
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
     const bool valid = threadIdx.x < BT && col < B;
@@ -569,10 +587,6 @@ static int launch_fwd_tma(const float* value, int64_t ldv, const float* reward, 
                           float* adv, int64_t lda, int64_t T, int64_t B, float gamma, float factor,
                           cudaStream_t stream, double* partials = nullptr, int* nblocks = nullptr,
                           const float* v_next = nullptr, float* carry = nullptr) {
-    using Pipe = ScanPipe<2, BT, TT, ST, 2>;
-    static SmemOptIn opt;
-    auto kernel = gae_fwd_tma<BT, TT, ST, MOM>;
-    if (int rc0 = opt.ensure(kernel, Pipe::kSmemBytes)) return rc0;
     TmapPack<2> maps;
     int rc = make_tmap_2d(&maps.m[0], value, T + 1, B, ldv, TT, BT);
     if (rc) return rc;
@@ -581,40 +595,28 @@ static int launch_fwd_tma(const float* value, int64_t ldv, const float* reward, 
     const unsigned grid = static_cast<unsigned>((B + BT - 1) / BT);
     if (nblocks) *nblocks = static_cast<int>(grid);
     if (v_next == nullptr) v_next = value + T * ldv;
-    kernel<<<grid, Pipe::kThreads, Pipe::kSmemBytes, stream>>>(maps, dtab, v_next, carry, adv, lda, static_cast<int>(T),
-                                                              static_cast<int>(B), gamma, factor, partials);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<2, 0, 0, BT, TT, ST, 2>, gae_fwd_tma<BT, TT, ST, MOM>>(
+        grid, stream, maps, dtab, v_next, carry, adv, lda, static_cast<int>(T), static_cast<int>(B), gamma, factor,
+        partials);
 }
 
 template <int BT, int TT, int ST>
 static int launch_bwd_tma(const float* grad_adv, int64_t ldg, const float* dtab, float* gv, int64_t ldgv, float* gr,
                           int64_t ldgr, int64_t T, int64_t B, float gamma, float factor, cudaStream_t stream,
                           float* carry = nullptr, int write_last = 1) {
-    using Pipe = ScanPipe<1, BT, TT, ST, 2>;
-    static SmemOptIn opt;
-    auto kernel = gae_bwd_tma<BT, TT, ST>;
-    if (int rc0 = opt.ensure(kernel, Pipe::kSmemBytes)) return rc0;
     TmapPack<1> maps;
     int rc = make_tmap_2d(&maps.m[0], grad_adv, T, B, ldg, TT, BT);
     if (rc) return rc;
     const unsigned grid = static_cast<unsigned>((B + BT - 1) / BT);
-    kernel<<<grid, Pipe::kThreads, Pipe::kSmemBytes, stream>>>(maps, dtab, gv, ldgv, gr, ldgr, static_cast<int>(T),
-                                                              static_cast<int>(B), gamma, factor, carry, write_last);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<1, 0, 0, BT, TT, ST, 2>, gae_bwd_tma<BT, TT, ST>>(
+        grid, stream, maps, dtab, gv, ldgv, gr, ldgr, static_cast<int>(T), static_cast<int>(B), gamma, factor, carry,
+        write_last);
 }
 
 template <int BT, int TT, int ST>
 static int launch_fwd_tma_st(const float* value, int64_t ldv, const float* reward, int64_t ldr, const float* dtab,
                              float* adv, int64_t lda, int64_t T, int64_t B, float gamma, float factor,
                              cudaStream_t stream, const float* v_next = nullptr, float* carry = nullptr) {
-    using Pipe = ScanPipeOut<2, 1, BT, TT, ST, 2>;
-    static SmemOptIn opt;
-    auto kernel = gae_fwd_tma_st<BT, TT, ST>;
-    if (int rc0 = opt.ensure(kernel, Pipe::kSmemBytes)) return rc0;
     TmapPack<2> maps;
     TmapPack<1> omaps;
     int rc = make_tmap_2d(&maps.m[0], value, T + 1, B, ldv, TT, BT);
@@ -625,21 +627,14 @@ static int launch_fwd_tma_st(const float* value, int64_t ldv, const float* rewar
     if (rc) return rc;
     const unsigned grid = static_cast<unsigned>((B + BT - 1) / BT);
     if (v_next == nullptr) v_next = value + T * ldv;
-    kernel<<<grid, Pipe::kThreads, Pipe::kSmemBytes, stream>>>(maps, omaps, dtab, v_next, carry, static_cast<int>(T),
-                                                              static_cast<int>(B), gamma, factor);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<2, 0, 1, BT, TT, ST, 2>, gae_fwd_tma_st<BT, TT, ST>>(
+        grid, stream, maps, omaps, dtab, v_next, carry, static_cast<int>(T), static_cast<int>(B), gamma, factor);
 }
 
 template <int BT, int TT, int ST>
 static int launch_bwd_tma_st(const float* grad_adv, int64_t ldg, const float* dtab, float* gv, int64_t ldgv, float* gr,
                              int64_t ldgr, int64_t T, int64_t B, float gamma, float factor, cudaStream_t stream,
                              float* carry = nullptr, int write_last = 1) {
-    using Pipe = ScanPipeOut<1, 2, BT, TT, ST, 2>;
-    static SmemOptIn opt;
-    auto kernel = gae_bwd_tma_st<BT, TT, ST>;
-    if (int rc0 = opt.ensure(kernel, Pipe::kSmemBytes)) return rc0;
     TmapPack<1> maps;
     TmapPack<2> omaps;
     int rc = make_tmap_2d(&maps.m[0], grad_adv, T, B, ldg, TT, BT);
@@ -649,11 +644,9 @@ static int launch_bwd_tma_st(const float* grad_adv, int64_t ldg, const float* dt
     rc = make_tmap_2d(&omaps.m[1], gr, T, B, ldgr, TT, BT);
     if (rc) return rc;
     const unsigned grid = static_cast<unsigned>((B + BT - 1) / BT);
-    kernel<<<grid, Pipe::kThreads, Pipe::kSmemBytes, stream>>>(maps, omaps, dtab, gv, ldgv, static_cast<int>(T),
-                                                              static_cast<int>(B), gamma, factor, carry, write_last);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<1, 0, 2, BT, TT, ST, 2>, gae_bwd_tma_st<BT, TT, ST>>(
+        grid, stream, maps, omaps, dtab, gv, ldgv, static_cast<int>(T), static_cast<int>(B), gamma, factor, carry,
+        write_last);
 }
 
 // Kernel regimes; hpc_rll_debug_set_config(HPC_RLL_OP_GAE, id) forces one, -1 picks by B.  <BT,TT,ST> = columns per

@@ -16,7 +16,7 @@
 // additive identity, so the first row is delta_{T-1} / G_0 exactly, signed zeros included (for gamma*lambda >= 0).
 //
 // Regimes (hpc_rll_debug_set_config(HPC_RLL_OP_GAE_EPISODIC, id) / HPC_RLL_CFG_GAE_EPISODIC force one):
-//   33 wide   ScanPipeMix (scan_pipe.cuh): value/next_value/reward and the two masks TMA-staged in (TT x BT) boxes,
+//   33 wide   ScanPipe (scan_pipe.cuh): value/next_value/reward and the two masks TMA-staged in (TT x BT) boxes,
 //             outputs TMA-stored.  Needs 16-byte aligned pointers and B % 16 == 0 with masks (a uint8 tensor map
 //             needs a 16-byte row stride), B % 4 == 0 without.
 //   21 look-back  single-launch T-split (scan_lookback.cuh), automatic for B <= 2048 and T >= 512.  The recurrence
@@ -62,15 +62,15 @@ __device__ __forceinline__ BwdOut bwd_step(float G, unsigned done, unsigned traj
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
-// wide path: ScanPipeMix.  NB = 2 reads both masks (a NULL one is replaced by the other's map and ignored through
-// has_done / has_traj), NB = 0 reads none.
+// wide path: ScanPipe with byte boxes.  NB = 2 reads both masks (a NULL one is replaced by the other's map and ignored
+// through has_done / has_traj), NB = 0 reads none.
 // ------------------------------------------------------------------------------------------------
 template <int NB>
 struct EpiFwdBody {
     float carry, g, gl;
     int has_done, has_traj;
-    __device__ __forceinline__ void step(int, const float (&x)[3], const unsigned (&m)[NB > 0 ? NB : 1],
-                                         float (&o)[1]) {
+    __device__ __forceinline__ void step(int, const float (&x)[3], const float (&)[1],
+                                         const unsigned (&m)[NB > 0 ? NB : 1], float (&o)[1]) {
         const unsigned d = NB > 0 && has_done ? m[0] : 0u;
         const unsigned tr = NB > 0 && has_traj ? m[NB > 1 ? 1 : 0] : 0u;
         float f;
@@ -82,17 +82,17 @@ template <int NB, int BT, int TT, int ST>
 __global__ void __launch_bounds__(BT + 32) gae_episodic_fwd_tma(const __grid_constant__ TmapPack<3 + NB> maps,
                                                                  const __grid_constant__ TmapPack<1> omaps, int T,
                                                                  float g, float gl, int has_done, int has_traj) {
-    using Pipe = ScanPipeMix<3, NB, 1, BT, TT, ST>;
+    using Pipe = ScanPipe<3, NB, 1, BT, TT, ST, 0>;
     EpiFwdBody<NB> body{-0.f, g, gl, has_done, has_traj};
-    Pipe::template run<true>(maps, omaps, T, blockIdx.x * BT, body);
+    Pipe::template run<true>(maps, omaps, nullptr, T, blockIdx.x * BT, body);
 }
 
 template <int NB>
 struct EpiBwdBody {
     float c, g, gl;
     int has_done, has_traj;
-    __device__ __forceinline__ void step(int, const float (&x)[1], const unsigned (&m)[NB > 0 ? NB : 1],
-                                         float (&o)[3]) {
+    __device__ __forceinline__ void step(int, const float (&x)[1], const float (&)[1],
+                                         const unsigned (&m)[NB > 0 ? NB : 1], float (&o)[3]) {
         const unsigned d = NB > 0 && has_done ? m[0] : 0u;
         const unsigned tr = NB > 0 && has_traj ? m[NB > 1 ? 1 : 0] : 0u;
         float f;
@@ -107,9 +107,9 @@ template <int NB, int BT, int TT, int ST>
 __global__ void __launch_bounds__(BT + 32) gae_episodic_bwd_tma(const __grid_constant__ TmapPack<1 + NB> maps,
                                                                  const __grid_constant__ TmapPack<3> omaps, int T,
                                                                  float g, float gl, int has_done, int has_traj) {
-    using Pipe = ScanPipeMix<1, NB, 3, BT, TT, ST>;
+    using Pipe = ScanPipe<1, NB, 3, BT, TT, ST, 0>;
     EpiBwdBody<NB> body{-0.f, g, gl, has_done, has_traj};
-    Pipe::template run<false>(maps, omaps, T, blockIdx.x * BT, body);
+    Pipe::template run<false>(maps, omaps, nullptr, T, blockIdx.x * BT, body);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -326,10 +326,6 @@ template <int NB>
 int launch_fwd_tma(const float* value, const float* next_value, const float* reward, const Masks& mk, float* adv,
                    int64_t T, int64_t B, float g, float gl, cudaStream_t stream) {
     constexpr int BT = kFwdBT, TT = kFwdTT;
-    using Pipe = ScanPipeMix<3, NB, 1, BT, TT, kFwdST>;
-    static SmemOptIn opt;
-    auto kernel = gae_episodic_fwd_tma<NB, BT, TT, kFwdST>;
-    if (int rc = opt.ensure(kernel, Pipe::kSmemBytes)) return rc;
     TmapPack<3 + NB> maps;
     TmapPack<1> omaps;
     const float* in[3] = {value, next_value, reward};
@@ -343,21 +339,14 @@ int launch_fwd_tma(const float* value, const float* next_value, const float* rew
     }
     if (int rc = make_tmap_2d(&omaps.m[0], adv, T, B, B, TT, BT)) return rc;
     const unsigned grid = static_cast<unsigned>((B + BT - 1) / BT);
-    kernel<<<grid, Pipe::kThreads, Pipe::kSmemBytes, stream>>>(maps, omaps, static_cast<int>(T), g, gl,
-                                                              mk.done != nullptr, mk.traj != nullptr);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<3, NB, 1, BT, TT, kFwdST, 0>, gae_episodic_fwd_tma<NB, BT, TT, kFwdST>>(
+        grid, stream, maps, omaps, static_cast<int>(T), g, gl, mk.done != nullptr, mk.traj != nullptr);
 }
 
 template <int NB>
 int launch_bwd_tma(const float* grad_adv, const Masks& mk, float* gv, float* gnv, float* gr, int64_t T, int64_t B,
                    float g, float gl, cudaStream_t stream) {
     constexpr int BT = kBwdBT, TT = kBwdTT;
-    using Pipe = ScanPipeMix<1, NB, 3, BT, TT, kBwdST>;
-    static SmemOptIn opt;
-    auto kernel = gae_episodic_bwd_tma<NB, BT, TT, kBwdST>;
-    if (int rc = opt.ensure(kernel, Pipe::kSmemBytes)) return rc;
     TmapPack<1 + NB> maps;
     TmapPack<3> omaps;
     if (int rc = make_tmap_2d(&maps.m[0], grad_adv, T, B, B, TT, BT)) return rc;
@@ -371,11 +360,8 @@ int launch_bwd_tma(const float* grad_adv, const Masks& mk, float* gv, float* gnv
     for (int k = 0; k < 3; ++k)
         if (int rc = make_tmap_2d(&omaps.m[k], out[k], T, B, B, TT, BT)) return rc;
     const unsigned grid = static_cast<unsigned>((B + BT - 1) / BT);
-    kernel<<<grid, Pipe::kThreads, Pipe::kSmemBytes, stream>>>(maps, omaps, static_cast<int>(T), g, gl,
-                                                              mk.done != nullptr, mk.traj != nullptr);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<1, NB, 3, BT, TT, kBwdST, 0>, gae_episodic_bwd_tma<NB, BT, TT, kBwdST>>(
+        grid, stream, maps, omaps, static_cast<int>(T), g, gl, mk.done != nullptr, mk.traj != nullptr);
 }
 
 int check_sizes(const char* what, int64_t T, int64_t B) {

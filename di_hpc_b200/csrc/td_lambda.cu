@@ -49,7 +49,7 @@ __global__ void __launch_bounds__(BT + 32) td_lambda_fwd_tma(const __grid_consta
                                                               float* __restrict__ grad_buf,
                                                               double* __restrict__ partials, int T, int B,
                                                               float gamma, float disc, float gmd, float neg_inv_n) {
-    using Pipe = ScanPipe<NIN, BT, TT, ST, 0>;
+    using Pipe = ScanPipe<NIN, 0, 0, BT, TT, ST, 0>;
     __shared__ double red[32];
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(BT + 32) td_lambda_fwd_tma(const __grid_consta
     body.t_last = T - 1;
     body.gbuf = grad_buf + static_cast<int64_t>(T - 1) * B + col;
     body.v1 = body.valid ? __ldg(value + static_cast<int64_t>(T) * B + col) : 0.f;
-    Pipe::template run<true>(maps, nullptr, T, col0, body);
+    Pipe::template run<true>(maps, {}, nullptr, T, col0, body);
     double v[1] = {body.valid ? body.acc : 0.0};
     block_sum<1>(v, red);
     if (threadIdx.x == 0) partials[blockIdx.x] = v[0];
@@ -178,10 +178,6 @@ template <int NIN, int BT, int TT, int ST>
 static int launch_tdl_tma(const float* value, const float* reward, const float* weight, float* grad_buf,
                           double* partials, int64_t T, int64_t B, float g, float disc, float gmd, float nin,
                           cudaStream_t stream, int* nblocks) {
-    using Pipe = ScanPipe<NIN, BT, TT, ST, 0>;
-    static SmemOptIn opt;
-    auto kernel = td_lambda_fwd_tma<NIN, BT, TT, ST>;
-    if (int rc0 = opt.ensure(kernel, Pipe::kSmemBytes)) return rc0;
     TmapPack<NIN> maps;
     int rc = make_tmap_2d(&maps.m[0], value, T + 1, B, B, TT, BT);
     if (rc) return rc;
@@ -193,11 +189,8 @@ static int launch_tdl_tma(const float* value, const float* reward, const float* 
     }
     const unsigned grid = static_cast<unsigned>((B + BT - 1) / BT);
     *nblocks = static_cast<int>(grid);
-    kernel<<<grid, Pipe::kThreads, Pipe::kSmemBytes, stream>>>(maps, value, grad_buf, partials, static_cast<int>(T),
-                                                              static_cast<int>(B), g, disc, gmd, nin);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<NIN, 0, 0, BT, TT, ST, 0>, td_lambda_fwd_tma<NIN, BT, TT, ST>>(
+        grid, stream, maps, value, grad_buf, partials, static_cast<int>(T), static_cast<int>(B), g, disc, gmd, nin);
 }
 
 // per-CTA loss partials: one per column tile, or one per (segment, tile) of the small-batch T-split (<= 4*SMs + tiles)

@@ -135,7 +135,7 @@ __global__ void __launch_bounds__(BT + 32) upgo_scan_tma(const __grid_constant__
                                                           const float* __restrict__ value, float* __restrict__ coef,
                                                           double* __restrict__ partials, int T, int B,
                                                           float neg_inv_n) {
-    using Pipe = ScanPipe<4, BT, TT, ST, 0>;
+    using Pipe = ScanPipe<4, 0, 0, BT, TT, ST, 0>;
     __shared__ double red[32];
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(BT + 32) upgo_scan_tma(const __grid_constant__
     body.t_last = T - 1;
     body.coef = coef + static_cast<int64_t>(T - 1) * B + col;
     body.v1 = body.valid ? __ldg(value + static_cast<int64_t>(T) * B + col) : 0.f;
-    Pipe::template run<true>(maps, nullptr, T, col0, body);
+    Pipe::template run<true>(maps, {}, nullptr, T, col0, body);
     double v[1] = {body.valid ? body.acc : 0.0};
     block_sum<1>(v, red);
     if (threadIdx.x == 0) partials[blockIdx.x] = v[0];
@@ -248,10 +248,6 @@ template <int BT, int TT, int ST>
 static int launch_upgo_scan(const float* value, const float* reward, const float* rho, const float* metric,
                             float* coef, double* partials, int64_t T, int64_t B, float nin, cudaStream_t stream,
                             int* nblocks) {
-    using Pipe = ScanPipe<4, BT, TT, ST, 0>;
-    static SmemOptIn opt;
-    auto kernel = upgo_scan_tma<BT, TT, ST>;
-    if (int rc0 = opt.ensure(kernel, Pipe::kSmemBytes)) return rc0;
     TmapPack<4> maps;
     const float* srcs[4] = {value, reward, rho, metric};
     for (int k = 0; k < 4; ++k) {
@@ -259,11 +255,9 @@ static int launch_upgo_scan(const float* value, const float* reward, const float
         if (rc1) return rc1;
     }
     *nblocks = static_cast<int>((B + BT - 1) / BT);
-    kernel<<<static_cast<unsigned>(*nblocks), Pipe::kThreads, Pipe::kSmemBytes, stream>>>(
-        maps, value, coef, partials, static_cast<int>(T), static_cast<int>(B), nin);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<4, 0, 0, BT, TT, ST, 0>, upgo_scan_tma<BT, TT, ST>>(
+        static_cast<unsigned>(*nblocks), stream, maps, value, coef, partials, static_cast<int>(T), static_cast<int>(B),
+        nin);
 }
 
 static inline int64_t align_up_(int64_t x, int64_t a) { return (x + a - 1) / a * a; }

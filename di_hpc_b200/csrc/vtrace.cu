@@ -227,7 +227,7 @@ __global__ void __launch_bounds__(BT + 32) vtrace_scan_tma(const __grid_constant
                                                             double* __restrict__ partials, int nblocks, int T, int B,
                                                             float gamma, float factor, float rc, float cc, float pc,
                                                             float inv_n) {
-    using Pipe = ScanPipe<NIN, BT, TT, ST, 0>;
+    using Pipe = ScanPipe<NIN, 0, 0, BT, TT, ST, 0>;
     __shared__ double red[64];
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
@@ -246,7 +246,7 @@ __global__ void __launch_bounds__(BT + 32) vtrace_scan_tma(const __grid_constant
     body.gv_buf = gv_buf + static_cast<int64_t>(T - 1) * B + col;
     body.v1 = body.valid ? __ldg(value + static_cast<int64_t>(T) * B + col) : 0.f;
     body.ret_next = body.v1;  // ret_T := v_T (vtrace.py:70)
-    Pipe::template run<true>(maps, nullptr, T, col0, body);
+    Pipe::template run<true>(maps, {}, nullptr, T, col0, body);
     double v[2] = {body.valid ? body.acc_pg : 0.0, body.valid ? body.acc_v : 0.0};
     block_sum<2>(v, red);
     if (threadIdx.x == 0) {
@@ -392,22 +392,15 @@ static int launch_vtrace_scan(const float* value, const float* reward, const flo
                               const float* weight, float* pg_coef, float* gv_buf, double* partials, int64_t T,
                               int64_t B, float g, float f, float rc, float cc, float pc, float inv_n,
                               cudaStream_t stream, int nblocks) {
-    using Pipe = ScanPipe<NIN, BT, TT, ST, 0>;
-    static SmemOptIn opt;
-    auto kernel = vtrace_scan_tma<NIN, BT, TT, ST>;
-    if (int rc0 = opt.ensure(kernel, Pipe::kSmemBytes)) return rc0;
     TmapPack<NIN> maps;
     const float* srcs[5] = {value, reward, is_in, logp_in, weight};
     for (int k = 0; k < NIN; ++k) {
         int rc1 = make_tmap_2d(&maps.m[k], srcs[k], k == 0 ? T + 1 : T, B, B, TT, BT);
         if (rc1) return rc1;
     }
-    kernel<<<static_cast<unsigned>(nblocks), Pipe::kThreads, Pipe::kSmemBytes, stream>>>(
-        maps, value, pg_coef, gv_buf, partials, nblocks, static_cast<int>(T), static_cast<int>(B), g, f, rc, cc, pc,
-        inv_n);
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
+    return launch_scan<ScanPipe<NIN, 0, 0, BT, TT, ST, 0>, vtrace_scan_tma<NIN, BT, TT, ST>>(
+        static_cast<unsigned>(nblocks), stream, maps, value, pg_coef, gv_buf, partials, nblocks, static_cast<int>(T),
+        static_cast<int>(B), g, f, rc, cc, pc, inv_n);
 }
 
 static inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }

@@ -2,6 +2,7 @@
 TMA tensor loads AND stores in the headline GAE kernels, bulk copies where the docs say so -- and no floating-point
 atomic anywhere (every reduction has a fixed order)."""
 import os
+import re
 import shutil
 import sys
 
@@ -67,3 +68,16 @@ def test_no_floating_point_atomics(sass):
             assert ".F32" not in op and ".F64" not in op and ".F16" not in op, (name, op)
         # the only kernels with atomics at all are the ticket / done counters of the look-back scans
         assert "lookback" in name, (name, sorted(ops))
+
+
+def test_against_compares_instruction_lines_with_anonymous_namespace_masked(sass, capsys):
+    from di_hpc_b200 import build
+    from tools import sass_opcodes
+    kernels, _, _ = sass
+    lib = build.build()
+    listing = sass_opcodes.listing(lib)
+    assert len(listing) == len(kernels)
+    assert sum(map(len, listing.values())) == sum(c["_total"] for c in kernels.values())
+    assert not [k for k in listing if re.search(r"_GLOBAL__N__[0-9a-f]{8}_", k)]
+    assert sass_opcodes.against(lib, lib) == 0
+    assert "instruction text differs: 0" in capsys.readouterr().out

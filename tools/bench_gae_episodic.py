@@ -5,7 +5,7 @@ normalised GAE module at the same shape as a bandwidth yardstick.
     python tools/bench_gae_episodic.py [--iters 200] [--warmup 20] [--out profiles/bench_gae_episodic_h100.json]
 
 Shapes (each selects one kernel regime, see csrc/gae_episodic.cu)
-  wide      T=1024, B=65536   TMA pipeline (ScanPipeMix)
+  wide      T=1024, B=65536   TMA pipeline (ScanPipe with uint8 mask boxes)
   lookback  T=1024, B=64      single-launch T-split with look-back
   generic   T=128,  B=1000    one column per thread (B % 16 != 0)
 Inputs: fp32 value / next_value / reward, a bool `done` with 1 % of entries set, traj_flag=None (= done).

@@ -24,7 +24,7 @@ def r(*s):
 
 
 def wide_and_fused():
-    """kernels added late in round 1: TMA-staged output (ScanPipeOut, config 33 = the default for wide batches),
+    """kernels added late in round 1: TMA-staged output (ScanPipe with NOUT > 0, config 33 = the default for wide batches),
     GAE with moments + PPO with fused normalisation, 64-bit / staged row paths (N = 18 / 9)"""
     T, B = 7, 40000
     v, rew = r(T + 1, B).requires_grad_(True), r(T, B).requires_grad_(True)
