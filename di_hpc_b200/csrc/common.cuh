@@ -208,6 +208,10 @@ __device__ __forceinline__ void st_stream2(float2* p, float2 v) { __stcs(p, v); 
 __device__ __forceinline__ void st_stream4(float4* p, float4 v) { __stcs(p, v); }
 __device__ __forceinline__ float ld_stream(const float* p) { return __ldcs(p); }
 __device__ __forceinline__ float4 ld_stream4(const float4* p) { return __ldcs(p); }
+// one byte of a mask tensor; a NULL mask reads as 0 (not set)
+__device__ __forceinline__ unsigned ld_mask(const uint8_t* __restrict__ p, int64_t i) {
+    return p != nullptr ? static_cast<unsigned>(__ldg(reinterpret_cast<const unsigned char*>(p) + i)) : 0u;
+}
 
 #endif  // __CUDACC__
 

@@ -172,6 +172,22 @@ struct GaeFwdBody {
     bool valid;
     double m1, m2;
     float p1, p2;  // fp32 partial moments of the current 16-row run, folded into m1/m2 at t % 16 == 0
+    // state at a segment edge: steps run from row t_edge-1 down, with g = g_{t_edge} (the carry) and
+    // v1 = v_row[col] (value row t_edge); `valid`: column col exists
+    static __device__ __forceinline__ GaeFwdBody at(int t_edge, float carry, const float* v_row, float* adv,
+                                                    int64_t ld, int col, float gamma, float factor, bool valid) {
+        GaeFwdBody b;
+        b.valid = valid;
+        b.g = carry;
+        b.gamma = gamma;
+        b.factor = factor;
+        b.ld = ld;
+        b.m1 = b.m2 = 0.0;
+        b.p1 = b.p2 = 0.f;
+        b.adv = adv + static_cast<int64_t>(t_edge - 1) * ld + col;
+        b.v1 = valid ? __ldg(v_row + col) : 0.f;
+        return b;
+    }
     __device__ __forceinline__ void step(int t, const float (&x)[2], const float (&dt)[2]) {
         const float a = fwd_step(x, dt, v1, gamma, factor, g);
         if (valid) st_stream(adv, a);
@@ -215,19 +231,9 @@ __global__ void __launch_bounds__(BT + 32) gae_fwd_tma(const __grid_constant__ T
     using Pipe = ScanPipe<2, 0, 0, BT, TT, ST, 2>;
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
-    GaeFwdBody<MOM> body;
-    body.valid = threadIdx.x < BT && col < B;
-    body.g = 0.f;
-    body.gamma = gamma;
-    body.factor = factor;
-    body.ld = ld_adv;
-    body.m1 = 0.0;
-    body.m2 = 0.0;
-    body.p1 = 0.f;
-    body.p2 = 0.f;
-    body.adv = adv + static_cast<int64_t>(T - 1) * ld_adv + col;
-    body.v1 = body.valid ? v_next[col] : 0.f;
-    if (carry != nullptr && body.valid) body.g = carry[col];
+    const bool valid = threadIdx.x < BT && col < B;
+    GaeFwdBody<MOM> body = GaeFwdBody<MOM>::at(T, 0.f, v_next, adv, ld_adv, col, gamma, factor, valid);
+    if (carry != nullptr && valid) body.g = carry[col];  // after at(): loading it first reorders the machine code
     Pipe::template run<true>(maps, {}, dtab, T, col0, body);
     if (carry != nullptr && body.valid) {
         carry[col] = body.g;
@@ -246,6 +252,22 @@ struct GaeBwdBody {
     int64_t ld_gv, ld_gr;
     bool valid;
     // gv / gr are running pointers (&grad[t][col] of the next step; t ascending)
+    // state at a segment edge: steps run from row t_edge up, with (gh, prev) = (ghat, dd) of row t_edge-1 (the carry)
+    static __device__ __forceinline__ GaeBwdBody at(int t_edge, float gh, float prev, float* gv, int64_t ld_gv,
+                                                    float* gr, int64_t ld_gr, int col, float gamma, float factor,
+                                                    bool valid) {
+        GaeBwdBody b;
+        b.valid = valid;
+        b.gh = gh;
+        b.prev = prev;
+        b.gamma = gamma;
+        b.factor = factor;
+        b.gv = gv + static_cast<int64_t>(t_edge) * ld_gv + col;
+        b.gr = gr + static_cast<int64_t>(t_edge) * ld_gr + col;
+        b.ld_gv = ld_gv;
+        b.ld_gr = ld_gr;
+        return b;
+    }
     __device__ __forceinline__ void step(int /*t*/, const float (&x)[1], const float (&dt)[2]) {
         const BwdOut o = bwd_step(x[0], dt, gamma, factor, gh, prev);
         if (valid) {
@@ -269,17 +291,9 @@ __global__ void __launch_bounds__(BT + 32) gae_bwd_tma(const __grid_constant__ T
     using Pipe = ScanPipe<1, 0, 0, BT, TT, ST, 2>;
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
-    GaeBwdBody body;
-    body.valid = threadIdx.x < BT && col < B;
-    body.gh = 0.f;
-    body.prev = 0.f;
-    body.gamma = gamma;
-    body.factor = factor;
-    body.gv = grad_value + col;
-    body.gr = grad_reward + col;
-    body.ld_gv = ld_gv;
-    body.ld_gr = ld_gr;
-    if (carry != nullptr && body.valid) {
+    const bool valid = threadIdx.x < BT && col < B;
+    GaeBwdBody body = GaeBwdBody::at(0, 0.f, 0.f, grad_value, ld_gv, grad_reward, ld_gr, col, gamma, factor, valid);
+    if (carry != nullptr && valid) {  // after at(): loading it first reorders the machine code
         body.gh = carry[col];
         body.prev = carry[B + col];
     }
@@ -359,9 +373,8 @@ __global__ void __launch_bounds__(BT + 32) gae_bwd_tma_st(const __grid_constant_
     }
 }
 
-// Generic (no alignment requirements) variants: one thread per column, plain coalesced loads with
-// a 4-deep software prefetch.  Used when a pointer / pitch is not 16-byte aligned so TMA cannot
-// describe the tensor.  Still a CUDA kernel -- there is no CPU path.
+// Generic (no alignment requirements) variants: the same bodies driven by scan_column (scan_pipe.cuh), one thread per
+// column.  Used when a pointer / pitch is not 16-byte aligned so TMA cannot describe the tensor.
 template <bool MOM>
 __global__ void __launch_bounds__(128) gae_fwd_generic(const float* __restrict__ value, int64_t ld_value,
                                                         const float* __restrict__ reward, int64_t ld_reward,
@@ -370,46 +383,12 @@ __global__ void __launch_bounds__(128) gae_fwd_generic(const float* __restrict__
                                                         double* __restrict__ partials,
                                                         const float* __restrict__ v_next, float* __restrict__ carry) {
     const int col = blockIdx.x * blockDim.x + threadIdx.x;
-    GaeFwdBody<MOM> body;
-    body.valid = col < B;
-    body.m1 = 0.0;
-    body.m2 = 0.0;
-    body.p1 = 0.f;
-    body.p2 = 0.f;
-    if (!MOM && !body.valid) return;
-    if (body.valid) {
-        body.g = 0.f;
-        body.gamma = gamma;
-        body.factor = factor;
-        body.ld = ld_adv;
-        body.adv = adv + static_cast<int64_t>(T - 1) * ld_adv + col;
-        body.v1 = v_next[col];
-        if (carry != nullptr) body.g = carry[col];
-        constexpr int U = 8;
-        int t = T - 1;
-        for (; t >= U - 1; t -= U) {
-            float v[U], r[U];
-            float2 d[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                v[u] = ld_stream(value + static_cast<int64_t>(t - u) * ld_value + col);
-                r[u] = ld_stream(reward + static_cast<int64_t>(t - u) * ld_reward + col);
-                d[u] = __ldg(reinterpret_cast<const float2*>(dtab) + t - u);
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const float x[2] = {v[u], r[u]};
-                const float dt[2] = {d[u].x, d[u].y};
-                body.step(t - u, x, dt);
-            }
-        }
-        for (; t >= 0; --t) {
-            const float x[2] = {value[static_cast<int64_t>(t) * ld_value + col],
-                                reward[static_cast<int64_t>(t) * ld_reward + col]};
-            const float2 d = __ldg(reinterpret_cast<const float2*>(dtab) + t);
-            const float dt[2] = {d.x, d.y};
-            body.step(t, x, dt);
-        }
+    const bool valid = col < B;
+    if (!MOM && !valid) return;
+    GaeFwdBody<MOM> body = GaeFwdBody<MOM>::at(T, carry != nullptr && valid ? carry[col] : 0.f, v_next, adv,
+                                               ld_adv, col, gamma, factor, valid);
+    if (valid) {
+        scan_column<2, 0, 0, 2, true>({{value, ld_value}, {reward, ld_reward}}, {}, dtab, {}, T, col, body);
         if (carry != nullptr) {
             carry[col] = body.g;
             carry[B + col] = body.v1;
@@ -429,39 +408,9 @@ __global__ void __launch_bounds__(128) gae_bwd_generic(const float* __restrict__
                                                         int write_last) {
     const int col = blockIdx.x * blockDim.x + threadIdx.x;
     if (col >= B) return;
-    GaeBwdBody body;
-    body.valid = true;
-    body.gh = carry != nullptr ? carry[col] : 0.f;
-    body.prev = carry != nullptr ? carry[B + col] : 0.f;
-    body.gamma = gamma;
-    body.factor = factor;
-    body.gv = grad_value + col;
-    body.gr = grad_reward + col;
-    body.ld_gv = ld_gv;
-    body.ld_gr = ld_gr;
-    constexpr int U = 8;
-    int t = 0;
-    for (; t + U <= T; t += U) {
-        float g[U];
-        float2 d[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            g[u] = ld_stream(grad_adv + static_cast<int64_t>(t + u) * ld_ga + col);
-            d[u] = __ldg(reinterpret_cast<const float2*>(dtab) + t + u);
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const float x[1] = {g[u]};
-            const float dt[2] = {d[u].x, d[u].y};
-            body.step(t + u, x, dt);
-        }
-    }
-    for (; t < T; ++t) {
-        const float x[1] = {grad_adv[static_cast<int64_t>(t) * ld_ga + col]};
-        const float2 d = __ldg(reinterpret_cast<const float2*>(dtab) + t);
-        const float dt[2] = {d.x, d.y};
-        body.step(t, x, dt);
-    }
+    GaeBwdBody body = GaeBwdBody::at(0, carry != nullptr ? carry[col] : 0.f, carry != nullptr ? carry[B + col] : 0.f,
+                                     grad_value, ld_gv, grad_reward, ld_gr, col, gamma, factor, true);
+    scan_column<1, 0, 0, 2, false>({{grad_adv, ld_ga}}, {}, dtab, {}, T, col, body);
     if (write_last) *body.gv = __fmul_rn(gamma, body.prev);  // row T
     if (carry != nullptr) {
         carry[col] = body.gh;
@@ -486,16 +435,9 @@ struct GaeFwdLbFac {
     float gamma, factor;
     using Body = GaeFwdBody<false>;
     __device__ __forceinline__ Body make(int pass, int t_edge, float carry) const {  // t_edge = row after the segment
-        Body b;
-        b.valid = valid && pass == 1;
-        b.g = carry;
-        b.gamma = gamma;
-        b.factor = factor;
-        b.ld = lda;
-        b.m1 = b.m2 = 0.0;
-        b.p1 = b.p2 = 0.f;
-        b.adv = adv + static_cast<int64_t>(t_edge - 1) * lda + col;
-        b.v1 = valid ? __ldg(value + static_cast<int64_t>(t_edge) * ldv + col) : 0.f;
+        const bool store = valid && pass == 1;
+        Body b = Body::at(t_edge, carry, value + static_cast<int64_t>(t_edge) * ldv, adv, lda, col, gamma, factor, valid);
+        b.valid = store;
         return b;
     }
     __device__ __forceinline__ void step(Body& b, int t, const float (&x)[2]) const {
@@ -537,18 +479,9 @@ struct GaeBwdLbFac {
     float gamma, factor;
     using Body = GaeBwdBody;
     __device__ __forceinline__ Body make(int pass, int t_edge, float carry) const {  // t_edge = first row of the segment
-        Body b;
-        b.valid = valid && pass == 1;
-        b.gh = carry;
         // dd of the previous row, exactly as the serial scan forms it: d_{t-1} * ghat_{t-1}
-        b.prev = t_edge > 0 ? __fmul_rn(__ldg(dtab + 2 * (t_edge - 1)), carry) : 0.f;
-        b.gamma = gamma;
-        b.factor = factor;
-        b.gv = gv + static_cast<int64_t>(t_edge) * ldgv + col;
-        b.gr = gr + static_cast<int64_t>(t_edge) * ldgr + col;
-        b.ld_gv = ldgv;
-        b.ld_gr = ldgr;
-        return b;
+        const float prev = t_edge > 0 ? __fmul_rn(__ldg(dtab + 2 * (t_edge - 1)), carry) : 0.f;
+        return Body::at(t_edge, carry, prev, gv, ldgv, gr, ldgr, col, gamma, factor, valid && pass == 1);
     }
     __device__ __forceinline__ void step(Body& b, int t, const float (&x)[1]) const {
         const float2 d = __ldg(reinterpret_cast<const float2*>(dtab) + t);

@@ -21,7 +21,8 @@
 //             needs a 16-byte row stride), B % 4 == 0 without.
 //   21 look-back  single-launch T-split (scan_lookback.cuh), automatic for B <= 2048 and T >= 512.  The recurrence
 //             has a per-element coefficient (CONSTA = false): each segment publishes A = prod f_t.
-//   99 generic one coalesced column per thread, 64-bit indexing: ragged B, misaligned pointers, short T.
+//   99 generic the wide bodies driven by scan_column (scan_pipe.cuh), one column per thread: ragged B, misaligned
+//             pointers, short T.
 // HBM traffic = algorithmic: forward 3 fp32 + 2 byte reads + 1 fp32 write = 18 B per element, backward 1 fp32 +
 // 2 byte reads + 3 fp32 writes = 18 B per element.  No atomics except the look-back tickets and counters.
 #include <cstdint>
@@ -113,12 +114,8 @@ __global__ void __launch_bounds__(BT + 32) gae_episodic_bwd_tma(const __grid_con
 }
 
 // ------------------------------------------------------------------------------------------------
-// generic path: one thread per column, 8 rows of loads in flight, 64-bit indexing throughout
+// generic path: the wide bodies driven by scan_column (scan_pipe.cuh); a NULL mask reads as 0
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned ld_mask(const uint8_t* __restrict__ p, int64_t i) {
-    return p != nullptr ? static_cast<unsigned>(__ldg(reinterpret_cast<const unsigned char*>(p) + i)) : 0u;
-}
-
 __global__ void __launch_bounds__(128) gae_episodic_fwd_generic(const float* __restrict__ value,
                                                                  const float* __restrict__ next_value,
                                                                  const float* __restrict__ reward,
@@ -128,30 +125,9 @@ __global__ void __launch_bounds__(128) gae_episodic_fwd_generic(const float* __r
                                                                  float g, float gl) {
     const int64_t col = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (col >= B) return;
-    float carry = -0.f, f;
-    constexpr int U = 8;
-    int64_t t = T - 1;
-    for (; t >= U - 1; t -= U) {
-        float v[U], nv[U], r[U];
-        unsigned d[U], tr[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const int64_t i = (t - u) * B + col;
-            v[u] = ld_stream(value + i);
-            nv[u] = ld_stream(next_value + i);
-            r[u] = ld_stream(reward + i);
-            d[u] = ld_mask(done, i);
-            tr[u] = ld_mask(traj, i);
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u)
-            st_stream(adv + (t - u) * B + col, fwd_step(v[u], nv[u], r[u], d[u], tr[u], g, gl, carry, f));
-    }
-    for (; t >= 0; --t) {
-        const int64_t i = t * B + col;
-        st_stream(adv + i, fwd_step(ld_stream(value + i), ld_stream(next_value + i), ld_stream(reward + i),
-                                    ld_mask(done, i), ld_mask(traj, i), g, gl, carry, f));
-    }
+    EpiFwdBody<2> body{-0.f, g, gl, 1, 1};
+    scan_column<3, 2, 1, 0, true>({{value, B}, {next_value, B}, {reward, B}}, {{done, B}, {traj, B}}, nullptr,
+                                  {{adv, B}}, T, col, body);
 }
 
 __global__ void __launch_bounds__(128) gae_episodic_bwd_generic(const float* __restrict__ grad_adv,
@@ -162,31 +138,9 @@ __global__ void __launch_bounds__(128) gae_episodic_bwd_generic(const float* __r
                                                                  float g, float gl) {
     const int64_t col = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (col >= B) return;
-    float c = -0.f, f;
-    constexpr int U = 8;
-    int64_t t = 0;
-    auto put = [&](int64_t i, const BwdOut& o) {
-        st_stream(gv + i, o.gv);
-        st_stream(gnv + i, o.gnv);
-        st_stream(gr + i, o.gr);
-    };
-    for (; t + U <= T; t += U) {
-        float G[U];
-        unsigned d[U], tr[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const int64_t i = (t + u) * B + col;
-            G[u] = ld_stream(grad_adv + i);
-            d[u] = ld_mask(done, i);
-            tr[u] = ld_mask(traj, i);
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) put((t + u) * B + col, bwd_step(G[u], d[u], tr[u], g, gl, c, f));
-    }
-    for (; t < T; ++t) {
-        const int64_t i = t * B + col;
-        put(i, bwd_step(ld_stream(grad_adv + i), ld_mask(done, i), ld_mask(traj, i), g, gl, c, f));
-    }
+    EpiBwdBody<2> body{-0.f, g, gl, 1, 1};
+    scan_column<1, 2, 3, 0, false>({{grad_adv, B}}, {{done, B}, {traj, B}}, nullptr, {{gv, B}, {gnv, B}, {gr, B}}, T,
+                                   col, body);
 }
 
 // ------------------------------------------------------------------------------------------------

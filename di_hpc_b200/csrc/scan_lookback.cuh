@@ -170,9 +170,11 @@ __device__ __forceinline__ void lb_stage(float* dst, const float* __restrict__ s
 }
 
 // Drives one segment: both passes over the chunks of rows [t0, t1), in scan order.
-//   Fac::make(pass, t_edge)  -> Body with its boundary state loaded (pass 1: zero carry, stores off)
-//   body.step(t, x, rt)      -> one step; x[k] = operand k at (t, col); Fac::table(t, rt) fills per-row constants
-//   Fac::state(body), Fac::coef(body) -> carried scalar / coefficient of the LAST step (ignored when CONSTA)
+//   Fac::make(pass, t_edge, carry) -> Body with its boundary state loaded at t_edge (t1 when REVERSE, else t0) and
+//                                     the carry; pass 0 gets carry 0 and must not store, pass 1 the folded carry
+//   Fac::step(body, t, x)          -> one step; x[k] = operand k at (t, col); Fac loads any per-row constants itself
+//   Fac::state(body), Fac::coef(body) -> carried scalar / coefficient of the LAST step (coef ignored when CONSTA)
+//   Fac::finish(body, t0, t1)      -> after pass 1: per-segment epilogue (e.g. loss partials, GAE's row T)
 template <int NIN, bool REVERSE, bool CONSTA, class Fac>
 __device__ __forceinline__ void lb_segment(const Fac& fac, const float* const (&in)[NIN], const int64_t (&ld)[NIN], int t0,
                                            int t1, int col, bool valid, const LbTile& lt, unsigned long long* words,

@@ -169,6 +169,64 @@ struct ScanPipe {
     }
 };
 
+// One operand of scan_column: base pointer and row pitch in elements.
+template <class P>
+struct ColOp {
+    P p;
+    int64_t ld;
+};
+
+// The generic regime of the same scans, for operands TMA cannot describe (misaligned pointers or pitches): the calling
+// thread walks column `col` over rows [0, T) in scan order with streaming loads, 8 rows in flight, 64-bit indexing.
+// The body is called as in ScanPipe::run, with x[k] = in[k] and m[k] = mk[k] (a NULL mask reads as 0) at (t, col),
+// rt[k] = rowtab[t*NTAB + k]; with NOUT > 0, o[k] is stored to out[k] at (t, col).
+template <int NF, int NB, int NOUT, int NTAB, bool REVERSE, class Body>
+__device__ __forceinline__ void scan_column(const ColOp<const float*> (&in)[NF],
+                                            const ColOp<const uint8_t*> (&mk)[NB > 0 ? NB : 1],
+                                            const float* __restrict__ rowtab,
+                                            const ColOp<float*> (&out)[NOUT > 0 ? NOUT : 1], int64_t T, int64_t col,
+                                            Body& body) {
+    static_assert(NTAB == 0 || NTAB == 2, "the row table is read as (d_t, 1/d_t) pairs");
+    constexpr int U = 8, kNB = NB > 0 ? NB : 1, kTabN = NTAB > 0 ? NTAB : 1;
+    const auto load = [&](int64_t t, float (&x)[NF], unsigned (&m)[kNB], float (&rt)[kTabN]) {
+#pragma unroll
+        for (int k = 0; k < NF; ++k) x[k] = ld_stream(in[k].p + t * in[k].ld + col);
+#pragma unroll
+        for (int k = 0; k < NB; ++k) m[k] = ld_mask(mk[k].p, t * mk[k].ld + col);
+        if constexpr (NTAB == 2) {
+            const float2 d = __ldg(reinterpret_cast<const float2*>(rowtab) + t);
+            rt[0] = d.x;
+            rt[1] = d.y;
+        }
+    };
+    const auto step = [&](int64_t t, const float (&x)[NF], const unsigned (&m)[kNB], const float (&rt)[kTabN]) {
+        if constexpr (NOUT == 0) {
+            body.step(static_cast<int>(t), x, rt);
+        } else {
+            float o[NOUT];
+            body.step(static_cast<int>(t), x, rt, m, o);
+#pragma unroll
+            for (int k = 0; k < NOUT; ++k) st_stream(out[k].p + t * out[k].ld + col, o[k]);
+        }
+    };
+    const auto row = [&](int64_t n) { return REVERSE ? T - 1 - n : n; };
+    int64_t n = 0;
+    for (; n + U <= T; n += U) {
+        float x[U][NF], rt[U][kTabN];
+        unsigned m[U][kNB];
+#pragma unroll
+        for (int u = 0; u < U; ++u) load(row(n + u), x[u], m[u], rt[u]);
+#pragma unroll
+        for (int u = 0; u < U; ++u) step(row(n + u), x[u], m[u], rt[u]);
+    }
+    for (; n < T; ++n) {
+        float x[NF], rt[kTabN];
+        unsigned m[kNB];
+        load(row(n), x, m, rt);
+        step(row(n), x, m, rt);
+    }
+}
+
 // Host: opts Kernel into Pipe's dynamic shared memory, launches it on `grid` CTAs of Pipe::kThreads and checks the
 // launch.  The opt-in record is keyed by the kernel itself: several scan kernels share one function type.
 template <class Pipe, auto Kernel, class... A>

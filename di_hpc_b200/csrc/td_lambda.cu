@@ -27,6 +27,25 @@ struct TdLambdaBody {
     int64_t ld;
     int t_last;
     bool valid;
+    // state at a segment edge: steps run from row t_edge-1 down, with ret = ret_{t_edge} (the carry; unused when
+    // t_edge = T) and v1 = value[t_edge]; `valid`: column col exists
+    static __device__ __forceinline__ TdLambdaBody at(int t_edge, float carry, const float* value, float* grad_buf,
+                                                      int B, int T, int col, float gamma, float disc, float gmd,
+                                                      float neg_inv_n, bool valid) {
+        TdLambdaBody b;
+        b.valid = valid;
+        b.ret = carry;
+        b.gamma = gamma;
+        b.disc = disc;
+        b.gmd = gmd;
+        b.neg_inv_n = neg_inv_n;
+        b.acc = 0.0;
+        b.ld = B;
+        b.t_last = T - 1;
+        b.gbuf = grad_buf + static_cast<int64_t>(t_edge - 1) * B + col;
+        b.v1 = valid ? __ldg(value + static_cast<int64_t>(t_edge) * B + col) : 0.f;
+        return b;
+    }
     __device__ __forceinline__ void step(int t, const float (&x)[NIN], const float (&)[1]) {
         // x[0] = v_t, x[1] = r_t, x[2] = w_t (if NIN == 3)
         if (t == t_last)
@@ -53,18 +72,8 @@ __global__ void __launch_bounds__(BT + 32) td_lambda_fwd_tma(const __grid_consta
     __shared__ double red[32];
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
-    TdLambdaBody<NIN> body;
-    body.valid = threadIdx.x < BT && col < B;
-    body.ret = 0.f;
-    body.gamma = gamma;
-    body.disc = disc;
-    body.gmd = gmd;
-    body.neg_inv_n = neg_inv_n;
-    body.acc = 0.0;
-    body.ld = B;
-    body.t_last = T - 1;
-    body.gbuf = grad_buf + static_cast<int64_t>(T - 1) * B + col;
-    body.v1 = body.valid ? __ldg(value + static_cast<int64_t>(T) * B + col) : 0.f;
+    TdLambdaBody<NIN> body = TdLambdaBody<NIN>::at(T, 0.f, value, grad_buf, B, T, col, gamma, disc, gmd, neg_inv_n,
+                                                   threadIdx.x < BT && col < B);
     Pipe::template run<true>(maps, {}, nullptr, T, col0, body);
     double v[1] = {body.valid ? body.acc : 0.0};
     block_sum<1>(v, red);
@@ -83,18 +92,9 @@ struct TdlLbFac {
     double* partial;  // this CTA's slot
     using Body = TdLambdaBody<NIN>;
     __device__ __forceinline__ Body make(int pass, int t_edge, float carry) const {
-        Body b;
-        b.valid = valid && pass == 1;
-        b.ret = carry;
-        b.gamma = gamma;
-        b.disc = disc;
-        b.gmd = gmd;
-        b.neg_inv_n = neg_inv_n;
-        b.acc = 0.0;
-        b.ld = B;
-        b.t_last = T - 1;
-        b.gbuf = grad_buf + static_cast<int64_t>(t_edge - 1) * B + col;
-        b.v1 = valid ? __ldg(value + static_cast<int64_t>(t_edge) * B + col) : 0.f;
+        const bool store = valid && pass == 1;
+        Body b = Body::at(t_edge, carry, value, grad_buf, B, T, col, gamma, disc, gmd, neg_inv_n, valid);
+        b.valid = store;
         return b;
     }
     __device__ __forceinline__ void step(Body& b, int t, const float (&x)[NIN]) const {
@@ -136,7 +136,7 @@ __global__ void __launch_bounds__(kLbCols) td_lambda_fwd_lookback(const float* _
     lb_end(ctl, S * tiles, lt.epoch);
 }
 
-// generic fallback (no TMA alignment requirements): one thread per column
+// generic fallback (no TMA alignment requirements): the same body driven by scan_column, one thread per column
 template <bool HAS_W>
 __global__ void __launch_bounds__(128) td_lambda_fwd_generic(const float* __restrict__ value,
                                                               const float* __restrict__ reward,
@@ -144,30 +144,15 @@ __global__ void __launch_bounds__(128) td_lambda_fwd_generic(const float* __rest
                                                               float* __restrict__ grad_buf,
                                                               double* __restrict__ partials, int T, int B,
                                                               float gamma, float disc, float gmd, float neg_inv_n) {
+    constexpr int NIN = HAS_W ? 3 : 2;
     __shared__ double red[32];
     const int col = blockIdx.x * blockDim.x + threadIdx.x;
-    TdLambdaBody<HAS_W ? 3 : 2> body;
-    body.valid = col < B;
-    body.ret = 0.f;
-    body.gamma = gamma;
-    body.disc = disc;
-    body.gmd = gmd;
-    body.neg_inv_n = neg_inv_n;
-    body.acc = 0.0;
-    body.ld = B;
-    body.t_last = T - 1;
-    body.gbuf = grad_buf + static_cast<int64_t>(T - 1) * B + col;
+    TdLambdaBody<NIN> body = TdLambdaBody<NIN>::at(T, 0.f, value, grad_buf, B, T, col, gamma, disc, gmd, neg_inv_n, col < B);
     if (body.valid) {
-        body.v1 = value[static_cast<int64_t>(T) * B + col];
-        const float none[1] = {0.f};
-        for (int t = T - 1; t >= 0; --t) {
-            const int64_t o = static_cast<int64_t>(t) * B + col;
-            float x[HAS_W ? 3 : 2];
-            x[0] = value[o];
-            x[1] = reward[o];
-            if (HAS_W) x[HAS_W ? 2 : 0] = weight[o];
-            body.step(t, x, none);
-        }
+        if constexpr (HAS_W)
+            scan_column<3, 0, 0, 0, true>({{value, B}, {reward, B}, {weight, B}}, {}, nullptr, {}, T, col, body);
+        else
+            scan_column<2, 0, 0, 0, true>({{value, B}, {reward, B}}, {}, nullptr, {}, T, col, body);
     }
     double v[1] = {body.valid ? body.acc : 0.0};
     block_sum<1>(v, red);

@@ -109,6 +109,25 @@ struct UpgoBody {
     int64_t ld;
     int t_last;
     bool valid;
+    // state at a segment edge: steps run from row t_edge-1 down, with ret = ret_{t_edge} (the carry; unused when
+    // t_edge = T), v1 = value[t_edge] and the history the first step looks at, r_{t_edge} and v_{t_edge+1} (rows that
+    // exist whenever t_edge < T; `reward` is not read at t_edge = T); `valid`: column col exists
+    static __device__ __forceinline__ UpgoBody at(int t_edge, float carry, const float* value, const float* reward,
+                                                  float* coef, int B, int T, int col, float neg_inv_n, bool valid) {
+        UpgoBody b;
+        b.valid = valid;
+        b.ret = carry;
+        b.neg_inv_n = neg_inv_n;
+        b.a_last = 1.f;
+        b.acc = 0.0;
+        b.ld = B;
+        b.t_last = T - 1;
+        b.coef = coef + static_cast<int64_t>(t_edge - 1) * B + col;
+        b.v1 = valid ? __ldg(value + static_cast<int64_t>(t_edge) * B + col) : 0.f;
+        b.v2 = (valid && t_edge < T) ? __ldg(value + static_cast<int64_t>(t_edge + 1) * B + col) : 0.f;
+        b.r1 = (valid && t_edge < T) ? __ldg(reward + static_cast<int64_t>(t_edge) * B + col) : 0.f;
+        return b;
+    }
     __device__ __forceinline__ void step(int t, const float (&x)[4], const float (&)[1]) {
         // x[0]=v_t x[1]=r_t x[2]=rho_t x[3]=metric_t
         const float v0 = x[0], r = x[1];
@@ -139,15 +158,7 @@ __global__ void __launch_bounds__(BT + 32) upgo_scan_tma(const __grid_constant__
     __shared__ double red[32];
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
-    UpgoBody body;
-    body.valid = threadIdx.x < BT && col < B;
-    body.ret = body.v2 = body.r1 = 0.f;
-    body.neg_inv_n = neg_inv_n;
-    body.acc = 0.0;
-    body.ld = B;
-    body.t_last = T - 1;
-    body.coef = coef + static_cast<int64_t>(T - 1) * B + col;
-    body.v1 = body.valid ? __ldg(value + static_cast<int64_t>(T) * B + col) : 0.f;
+    UpgoBody body = UpgoBody::at(T, 0.f, value, nullptr, coef, B, T, col, neg_inv_n, threadIdx.x < BT && col < B);
     Pipe::template run<true>(maps, {}, nullptr, T, col0, body);
     double v[1] = {body.valid ? body.acc : 0.0};
     block_sum<1>(v, red);
@@ -166,19 +177,9 @@ struct UpgoLbFac {
     double* partial;
     using Body = UpgoBody;
     __device__ __forceinline__ Body make(int pass, int t_edge, float carry) const {
-        Body b;
-        b.valid = valid && pass == 1;
-        b.ret = carry;
-        b.neg_inv_n = neg_inv_n;
-        b.a_last = 1.f;
-        b.acc = 0.0;
-        b.ld = B;
-        b.t_last = T - 1;
-        b.coef = coef_out + static_cast<int64_t>(t_edge - 1) * B + col;
-        b.v1 = valid ? __ldg(value + static_cast<int64_t>(t_edge) * B + col) : 0.f;
-        // history the first step of the segment looks at: r_{t+1}, v_{t+2} (rows that exist whenever t_edge < T)
-        b.v2 = (valid && t_edge < T) ? __ldg(value + static_cast<int64_t>(t_edge + 1) * B + col) : 0.f;
-        b.r1 = (valid && t_edge < T) ? __ldg(reward + static_cast<int64_t>(t_edge) * B + col) : 0.f;
+        const bool store = valid && pass == 1;
+        Body b = Body::at(t_edge, carry, value, reward, coef_out, B, T, col, neg_inv_n, valid);
+        b.valid = store;
         return b;
     }
     __device__ __forceinline__ void step(Body& b, int t, const float (&x)[4]) const {
@@ -222,23 +223,9 @@ __global__ void __launch_bounds__(128) upgo_scan_generic(const float* __restrict
                                                           float neg_inv_n) {
     __shared__ double red[32];
     const int col = blockIdx.x * blockDim.x + threadIdx.x;
-    UpgoBody body;
-    body.valid = col < B;
-    body.ret = body.v2 = body.r1 = 0.f;
-    body.neg_inv_n = neg_inv_n;
-    body.acc = 0.0;
-    body.ld = B;
-    body.t_last = T - 1;
-    body.coef = coef + static_cast<int64_t>(T - 1) * B + col;
-    if (body.valid) {
-        body.v1 = value[static_cast<int64_t>(T) * B + col];
-        const float none[1] = {0.f};
-        for (int t = T - 1; t >= 0; --t) {
-            const int64_t o = static_cast<int64_t>(t) * B + col;
-            const float x[4] = {value[o], reward[o], rho[o], metric[o]};
-            body.step(t, x, none);
-        }
-    }
+    UpgoBody body = UpgoBody::at(T, 0.f, value, nullptr, coef, B, T, col, neg_inv_n, col < B);
+    if (body.valid)
+        scan_column<4, 0, 0, 0, true>({{value, B}, {reward, B}, {rho, B}, {metric, B}}, {}, nullptr, {}, T, col, body);
     double v[1] = {body.valid ? body.acc : 0.0};
     block_sum<1>(v, red);
     if (threadIdx.x == 0) partials[blockIdx.x] = v[0];

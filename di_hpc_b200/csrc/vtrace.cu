@@ -195,6 +195,29 @@ struct VtraceBody {
     float* gv_buf;
     int64_t ld;
     bool valid;
+    // state at a segment edge: steps run from row t_edge-1 down, with item = item_{t_edge} (the carry), v1 = value[t_edge]
+    // and ret_next = v1 + item (ret_T := v_T, vtrace.py:70); `valid`: column col exists
+    static __device__ __forceinline__ VtraceBody at(int t_edge, float carry, const float* value, float* pg_coef,
+                                                    float* gv_buf, int B, int T, int col, float gamma, float factor,
+                                                    float rc, float cc, float pc, float inv_n, bool valid) {
+        VtraceBody b;
+        b.valid = valid;
+        b.item = carry;
+        b.gamma = gamma;
+        b.factor = factor;
+        b.rc = rc;
+        b.cc = cc;
+        b.pc = pc;
+        b.inv_n = inv_n;
+        b.a_last = 1.f;
+        b.acc_pg = b.acc_v = 0.0;
+        b.ld = B;
+        b.pg_coef = pg_coef + static_cast<int64_t>(t_edge - 1) * B + col;
+        b.gv_buf = gv_buf + static_cast<int64_t>(t_edge - 1) * B + col;
+        b.v1 = valid ? __ldg(value + static_cast<int64_t>(t_edge) * B + col) : 0.f;
+        b.ret_next = t_edge < T ? __fadd_rn(b.v1, carry) : b.v1;
+        return b;
+    }
     __device__ __forceinline__ void step(int /*t*/, const float (&x)[NIN], const float (&)[1]) {
         // x[0]=v_t x[1]=r_t x[2]=IS_t x[3]=logp_t x[4]=w_t
         const float is = x[2];
@@ -231,21 +254,8 @@ __global__ void __launch_bounds__(BT + 32) vtrace_scan_tma(const __grid_constant
     __shared__ double red[64];
     const int col0 = blockIdx.x * BT;
     const int col = col0 + threadIdx.x;
-    VtraceBody<NIN> body;
-    body.valid = threadIdx.x < BT && col < B;
-    body.item = 0.f;
-    body.gamma = gamma;
-    body.factor = factor;
-    body.rc = rc;
-    body.cc = cc;
-    body.pc = pc;
-    body.inv_n = inv_n;
-    body.acc_pg = body.acc_v = 0.0;
-    body.ld = B;
-    body.pg_coef = pg_coef + static_cast<int64_t>(T - 1) * B + col;
-    body.gv_buf = gv_buf + static_cast<int64_t>(T - 1) * B + col;
-    body.v1 = body.valid ? __ldg(value + static_cast<int64_t>(T) * B + col) : 0.f;
-    body.ret_next = body.v1;  // ret_T := v_T (vtrace.py:70)
+    VtraceBody<NIN> body = VtraceBody<NIN>::at(T, 0.f, value, pg_coef, gv_buf, B, T, col, gamma, factor, rc, cc, pc,
+                                               inv_n, threadIdx.x < BT && col < B);
     Pipe::template run<true>(maps, {}, nullptr, T, col0, body);
     double v[2] = {body.valid ? body.acc_pg : 0.0, body.valid ? body.acc_v : 0.0};
     block_sum<2>(v, red);
@@ -269,6 +279,8 @@ struct VtraceLbFac {
     double* partial_pg;
     double* partial_v;
     using Body = VtraceBody<NIN>;
+    // not VtraceBody::at: its t_edge < T test for ret_next changes this kernel's machine code.  The carry is 0 at
+    // t_edge = T, so v1 + carry here equals at()'s v1 up to the sign of a zero.
     __device__ __forceinline__ Body make(int pass, int t_edge, float carry) const {
         Body b;
         b.valid = valid && pass == 1;
@@ -351,33 +363,15 @@ __global__ void __launch_bounds__(128) vtrace_scan_generic(const float* __restri
                                                             float inv_n) {
     __shared__ double red[64];
     const int col = blockIdx.x * blockDim.x + threadIdx.x;
-    VtraceBody<HAS_W ? 5 : 4> body;
-    body.valid = col < B;
-    body.item = 0.f;
-    body.gamma = gamma;
-    body.factor = factor;
-    body.rc = rc;
-    body.cc = cc;
-    body.pc = pc;
-    body.inv_n = inv_n;
-    body.acc_pg = body.acc_v = 0.0;
-    body.ld = B;
-    body.pg_coef = pg_coef + static_cast<int64_t>(T - 1) * B + col;
-    body.gv_buf = gv_buf + static_cast<int64_t>(T - 1) * B + col;
+    VtraceBody<HAS_W ? 5 : 4> body = VtraceBody<HAS_W ? 5 : 4>::at(T, 0.f, value, pg_coef, gv_buf, B, T, col, gamma,
+                                                                   factor, rc, cc, pc, inv_n, col < B);
     if (body.valid) {
-        body.v1 = value[static_cast<int64_t>(T) * B + col];
-        body.ret_next = body.v1;
-        const float none[1] = {0.f};
-        for (int t = T - 1; t >= 0; --t) {
-            const int64_t o = static_cast<int64_t>(t) * B + col;
-            float x[HAS_W ? 5 : 4];
-            x[0] = value[o];
-            x[1] = reward[o];
-            x[2] = is_in[o];
-            x[3] = logp_in[o];
-            if (HAS_W) x[HAS_W ? 4 : 0] = weight[o];
-            body.step(t, x, none);
-        }
+        if constexpr (HAS_W)
+            scan_column<5, 0, 0, 0, true>({{value, B}, {reward, B}, {is_in, B}, {logp_in, B}, {weight, B}}, {}, nullptr,
+                                          {}, T, col, body);
+        else
+            scan_column<4, 0, 0, 0, true>({{value, B}, {reward, B}, {is_in, B}, {logp_in, B}}, {}, nullptr, {}, T, col,
+                                          body);
     }
     double v[2] = {body.valid ? body.acc_pg : 0.0, body.valid ? body.acc_v : 0.0};
     block_sum<2>(v, red);

@@ -2,6 +2,9 @@
 fixtures, at the reference test shape, a large sparse map and edge shapes; both backward regimes; out-of-range
 locations with guard bands; run-to-run and layout invariance; the legacy names; CUDA-graph replay; > 2^31 elements."""
 import ctypes
+import os
+import subprocess
+import sys
 
 import numpy as np
 import pytest
@@ -10,6 +13,7 @@ import torch
 from tests._golden import GOLDEN_DIR, names
 
 pytestmark = pytest.mark.gpu
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(autouse=True)
@@ -88,10 +92,19 @@ def test_edge_shapes(B, M, N, H, W, kw):
 
 
 def backward_kernels(B, M, N, H, W):
-    x, loc, G = inputs(B, M, N, H, W, 5)
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        module_run(x, loc, G, H, W, "add")
-    return {e.name for e in prof.events() if "scatter_conn_bwd" in e.name}
+    """Names of the backward kernels one module call launches.  Profiled in a fresh process: late in a long GPU run in
+    one process, torch.profiler sessions have come back with no CUDA events at all."""
+    code = "\n".join([
+        "import torch",
+        "from tests.test_scatter_connection_gpu import inputs, module_run",
+        "x, loc, G = inputs(%d, %d, %d, %d, %d, 5)" % (B, M, N, H, W),
+        "with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:",
+        "    module_run(x, loc, G, %d, %d, 'add')" % (H, W),
+        "print('\\n'.join({e.name for e in prof.events() if 'scatter_conn_bwd' in e.name}))"])
+    flags = ["-s"] if sys.flags.no_user_site else []
+    r = subprocess.run([sys.executable, *flags, "-c", code], cwd=ROOT, capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    return set(r.stdout.splitlines())
 
 
 @pytest.mark.parametrize("M,dense", [(64, True), (8, False)])
