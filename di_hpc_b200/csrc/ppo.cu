@@ -87,10 +87,46 @@ constexpr int ppo_min_blocks(int kmax, int width) {
     return ne >= 32 ? 1 : ((ne >= 20 || (ne == 8 && kmax >= 4)) ? 2 : 3);
 }
 
-// G1: one lane per row (G == 1, N == KMAX * WIDTH exactly) known at compile time -- the group loops, the `e0 < N`
-// predicates and the element-index arithmetic of the row helpers fold away (the kernel is bound by instruction issue
-// at small N).
-template <int KMAX, int WIDTH, bool G1 = false>
+// staged and looping layouts: one (new, old) logits row pair and the sample's scalars -> the five loss terms and the
+// two backward coefficients; args: (action, value_new, value_old, adv, ret, weight, pol_coef, val_coef, &P)
+struct PpoRowOp {
+    static constexpr int kTensors = 2;
+    static constexpr bool kEntropy = true, kCat = true;
+    struct Scalars {
+        float adv, vn, vo, ret, w;
+        int a;
+    };
+    double acc[5];
+    const AdvNorm norm;
+    __device__ __forceinline__ Scalars scalars(int64_t r, bool, int, const int64_t* __restrict__ action,
+                                               const float* __restrict__ value_new,
+                                               const float* __restrict__ value_old, const float* __restrict__ adv,
+                                               const float* __restrict__ ret, const float* __restrict__ weight, float*,
+                                               float*, const PpoParams*) const {
+        Scalars sc;
+        sc.a = static_cast<int>(action[r]);
+        sc.adv = adv[r];
+        sc.vn = value_new[r];
+        sc.vo = value_old[r];
+        sc.ret = ret[r];
+        sc.w = weight ? weight[r] : 1.f;
+        return sc;
+    }
+    __device__ __forceinline__ void emit(int64_t row, const Scalars& sc, float H, float lp0, float lp1, const int64_t*,
+                                         const float*, const float*, const float*, const float*, const float*,
+                                         float* __restrict__ pol_coef, float* __restrict__ val_coef,
+                                         const PpoParams* P) {
+        float pc, vc;
+        ppo_sample(*P, lp0, lp1, H, norm(sc.adv), sc.vn, sc.vo, sc.ret, sc.w, acc, pc, vc);
+        pol_coef[row] = pc;
+        val_coef[row] = vc;
+    }
+};
+
+// The register layout keeps its own walk rather than HPC_ROWS_FWD_REGS: through the shared walk this kernel's machine
+// code changes (register assignment in every layout, register counts and spills in some), whatever the shape of the op.
+// G1: see HPC_ROWS_FWD_REGS.
+template <int KMAX, int WIDTH, bool G1>
 __global__ void __launch_bounds__(256, ppo_min_blocks(KMAX, WIDTH)) ppo_rows_fwd(const float* __restrict__ logits_new,
                                                      const float* __restrict__ logits_old,
                                                      const int64_t* __restrict__ action,
@@ -109,7 +145,7 @@ __global__ void __launch_bounds__(256, ppo_min_blocks(KMAX, WIDTH)) ppo_rows_fwd
     const int rows_per_block = rows_per_warp * 8;
     double acc[5] = {0, 0, 0, 0, 0};
     const AdvNorm norm(P);
-    constexpr bool PF = Row::NE <= 8;  // software pipeline (see softmax_rows.cu)
+    constexpr bool PF = Row::NE <= 8;  // software pipeline (see HPC_ROWS_FWD_REGS)
     Row rn, ro, nn, no;
     // per-sample scalars travel with the row loads (one iteration ahead), so that their latency is not exposed a
     // second time after the row statistics (ncu: this kernel was long-scoreboard-bound, 5.8 of 10 stall cycles)
@@ -181,47 +217,16 @@ __global__ void __launch_bounds__(256, ppo_min_blocks(KMAX, WIDTH)) ppo_rows_fwd
     }
 }
 
-// staged variant (N <= 32, not 128-bit eligible): see softmax_rows.cuh "Staged rows"
 __global__ void __launch_bounds__(kStageRows) ppo_rows_fwd_staged(
     const float* __restrict__ logits_new, const float* __restrict__ logits_old, const int64_t* __restrict__ action,
     const float* __restrict__ value_new, const float* __restrict__ value_old, const float* __restrict__ adv,
     const float* __restrict__ ret, const float* __restrict__ weight, float* __restrict__ pol_coef,
     float* __restrict__ val_coef, double* __restrict__ partials, const PpoParams P, int64_t R, int N, int pitch,
     int aligned) {
-    extern __shared__ float tiles[];
-    __shared__ double red[5 * 32];
-    float* tn = tiles;
-    float* to = tiles + kStageRows * pitch;
-    double acc[5] = {0, 0, 0, 0, 0};
-    const AdvNorm norm(P);
-    const int64_t ntiles = (R + kStageRows - 1) / kStageRows;
-    for (int64_t tix = blockIdx.x; tix < ntiles; tix += gridDim.x) {
-        const int64_t row0 = tix * kStageRows, row = row0 + threadIdx.x;
-        __syncthreads();
-        stage_rows(logits_new, R, N, pitch, row0, tn, aligned != 0);
-        stage_rows(logits_old, R, N, pitch, row0, to, aligned != 0);
-        __syncthreads();
-        if (row < R) {
-            const float* xn = tn + threadIdx.x * pitch;
-            const float* xo = to + threadIdx.x * pitch;
-            float mn, sn, t1, mo, so, t2;
-            staged_stats<true>(xn, N, mn, sn, t1);
-            staged_stats<false>(xo, N, mo, so, t2);
-            const float lsn = logf(sn), lso = logf(so);
-            const float H = lsn - t1 / sn;
-            const int a = static_cast<int>(action[row]);
-            float pc, vc;
-            ppo_sample(P, row_logp<true>(xn[a], mn, lsn), row_logp<true>(xo[a], mo, lso), H, norm(adv[row]),
-                       value_new[row], value_old[row], ret[row], weight ? weight[row] : 1.f, acc, pc, vc);
-            pol_coef[row] = pc;
-            val_coef[row] = vc;
-        }
-    }
-    block_sum<5>(acc, red);
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int k = 0; k < 5; ++k) partials[static_cast<size_t>(k) * gridDim.x + blockIdx.x] = acc[k];
-    }
+    PpoRowOp op{{0, 0, 0, 0, 0}, AdvNorm(P)};
+    rows_fwd_staged(op, R, N, pitch, aligned, logits_new, logits_old, action, value_new, value_old, adv, ret, weight,
+                    pol_coef, val_coef, &P);
+    flush_partials(op.acc, partials);
 }
 
 __global__ void __launch_bounds__(256) ppo_rows_fwd_loop(const float* __restrict__ logits_new,
@@ -234,49 +239,19 @@ __global__ void __launch_bounds__(256) ppo_rows_fwd_loop(const float* __restrict
                                                           float* __restrict__ pol_coef, float* __restrict__ val_coef,
                                                           double* __restrict__ partials, const PpoParams P, int64_t R,
                                                           int N) {
-    __shared__ double red[5 * 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    double acc[5] = {0, 0, 0, 0, 0};
-    const AdvNorm norm(P);
-    for (int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + warp; row < R; row += static_cast<int64_t>(gridDim.x) * 8) {
-        const float* xn = logits_new + row * N;
-        const float* xo = logits_old + row * N;
-        float mn = -INFINITY, mo = -INFINITY;
-        for (int k = lane; k < N; k += 32) {
-            mn = fmaxf(mn, xn[k]);
-            mo = fmaxf(mo, xo[k]);
-        }
-        mn = warp_max(mn);
-        mo = warp_max(mo);
-        float sn = 0.f, so = 0.f;
-        for (int k = lane; k < N; k += 32) {
-            sn += exp_term(xn[k] - mn);
-            so += exp_term(xo[k] - mo);
-        }
-        sn = warp_sum(sn);
-        so = warp_sum(so);
-        const float lsn = logf(sn), lso = logf(so);
-        float h = 0.f;
-        for (int k = lane; k < N; k += 32) {
-            const float lp = fmaxf(row_logp<true>(xn[k], mn, lsn), kNegBig);  // -inf logits: 0 * -3e38, not NaN
-            h += exp_term(lp) * lp;
-        }
-        const float H = -warp_sum(h);
-        if (lane == 0) {
-            const int a = static_cast<int>(action[row]);
-            float pc, vc;
-            ppo_sample(P, row_logp<true>(xn[a], mn, lsn), row_logp<true>(xo[a], mo, lso), H, norm(adv[row]),
-                       value_new[row], value_old[row], ret[row], weight ? weight[row] : 1.f, acc, pc, vc);
-            pol_coef[row] = pc;
-            val_coef[row] = vc;
-        }
-    }
-    block_sum<5>(acc, red);
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int k = 0; k < 5; ++k) partials[static_cast<size_t>(k) * gridDim.x + blockIdx.x] = acc[k];
-    }
+    PpoRowOp op{{0, 0, 0, 0, 0}, AdvNorm(P)};
+    rows_fwd_loop(op, R, N, logits_new, logits_old, action, value_new, value_old, adv, ret, weight, pol_coef, val_coef,
+                  &P);
+    flush_partials(op.acc, partials);
 }
+
+struct PpoRows {
+    template <int K, int W, bool G1>
+    static auto reg() { return ppo_rows_fwd<K, W, G1>; }
+    static auto staged() { return ppo_rows_fwd_staged; }
+    static auto loop() { return ppo_rows_fwd_loop; }
+    static constexpr int kStagedTiles = 2;
+};
 
 size_t ppo_workspace_bytes() { return static_cast<size_t>(sm_count()) * 16 * 5 * 8 + 256; }
 
@@ -305,37 +280,10 @@ static int ppo_forward_impl(const float* logits_new, const float* logits_old, co
     P.inv_n = static_cast<float>(inv_n);
     P.adv_stats = adv_stats;
     double* partials = static_cast<double*>(workspace);
-    const RowGeom ge = row_geom(N, logits_new, logits_old);
-    int log2G = 0;
-    while ((1 << log2G) < ge.G) ++log2G;
-    const bool staged = use_staged_rows(N, ge.width);
-    const unsigned grid = rows_grid(B, staged ? kStageRows : (ge.kmax == 0 ? 8 : (32 / ge.G) * 8));
-    const int n = static_cast<int>(N);
-#define HPC_PPO_ROWS(K, V)                                                                                          \
-    do {                                                                                                            \
-        if (ge.G == 1)                                                                                              \
-            ppo_rows_fwd<K, V, true><<<grid, 256, 0, stream>>>(logits_new, logits_old, action, value_new, value_old, \
-                                                               adv, return_, weight, pol_coef, val_coef, partials, P, \
-                                                               B, n, 1, 0);                                           \
-        else                                                                                                        \
-            ppo_rows_fwd<K, V, false><<<grid, 256, 0, stream>>>(logits_new, logits_old, action, value_new,           \
-                                                                value_old, adv, return_, weight, pol_coef, val_coef, \
-                                                                partials, P, B, n, ge.G, log2G);                     \
-    } while (0)
-    if (staged) {
-        static SmemOptIn opt;
-        if (int rc0 = opt.ensure(ppo_rows_fwd_staged, static_cast<int>(stage_bytes(32, 2)))) return rc0;  // largest pitch (N=32 -> 33)
-        ppo_rows_fwd_staged<<<grid, kStageRows, stage_bytes(n, 2), stream>>>(
-            logits_new, logits_old, action, value_new, value_old, adv, return_, weight, pol_coef, val_coef, partials, P, B,
-            n, stage_pitch(n), aligned16(logits_new) && aligned16(logits_old) ? 1 : 0);
-    } else if (ge.kmax == 0)
-        ppo_rows_fwd_loop<<<grid, 256, 0, stream>>>(logits_new, logits_old, action, value_new, value_old, adv, return_,
-                                                    weight, pol_coef, val_coef, partials, P, B, n);
-    else
-        HPC_ROW_DISPATCH(ge, HPC_PPO_ROWS);
-#undef HPC_PPO_ROWS
-    count_launch();
-    HPC_LAUNCH_CHECK();
+    unsigned grid;
+    if (int rc = launch_rows<PpoRows>(&grid, B, N, logits_new, logits_old, stream, logits_new, logits_old, action,
+                                      value_new, value_old, adv, return_, weight, pol_coef, val_coef, partials, P))
+        return rc;
     FinSpec spec;
     const double sc[5] = {inv_n, 0.5 * inv_n, inv_n, inv_n, inv_n};
     for (int k = 0; k < 5; ++k) {
@@ -389,7 +337,7 @@ int hpc_rll_ppo_backward(const float* grad_policy_loss, const float* grad_value_
     if (global_B <= 0) global_B = B;
     const double inv_n = 1.0 / static_cast<double>(global_B);
     int rc = launch_softmax_grad_rows(logits_new, action, pol_coef, weight, grad_policy_loss, grad_entropy_loss, inv_n,
-                                      grad_logits_new, B, N, true, stream);
+                                      grad_logits_new, B, N, stream);
     if (rc) return rc;
     return launch_scale_copy(val_coef, grad_value_loss, grad_value_new, B, 0, stream);
 }

@@ -8,8 +8,11 @@
 
 namespace hpcrll {
 
-// G1: one lane per row known at compile time (G == 1, N == KMAX * WIDTH): see ppo_rows_fwd
-template <int KMAX, int WIDTH, bool ENT, bool CAT, bool G1 = false>
+// The backward writes a whole row where the forwards reduce it to scalars, so it keeps its own three kernels.  They
+// always carry the entropy term; a caller without one passes a zero coefficient (launch_softmax_grad_rows).
+
+// G1: one lane per row known at compile time (G == 1, N == KMAX * WIDTH): see HPC_ROWS_FWD_REGS
+template <int KMAX, int WIDTH, bool G1>
 __global__ void __launch_bounds__(256) softmax_grad_rows_kernel(const float* __restrict__ logits,
                                                                  const int64_t* __restrict__ action,
                                                                  const float* __restrict__ c1,
@@ -26,7 +29,7 @@ __global__ void __launch_bounds__(256) softmax_grad_rows_kernel(const float* __r
     const int rows_per_warp = 32 >> log2G;
     const int rows_per_block = rows_per_warp * 8;
     const float s1 = __ldg(g1);
-    const float s2 = ENT ? __ldg(g2) * inv_n : 0.f;
+    const float s2 = __ldg(g2) * inv_n;
     // software pipeline (small rows only): the next row block's loads fly while this one is reduced
     constexpr bool PF = Row::NE <= 8;
     Row rr, nx;
@@ -45,10 +48,10 @@ __global__ void __launch_bounds__(256) softmax_grad_rows_kernel(const float* __r
         if (PF) nx.load(pl, N, G, lig, nrow < R);
         const int a = active ? static_cast<int>(action[row]) : -1;
         const float c = active ? s1 * c1[row] : 0.f;
-        const float e2 = ENT ? s2 * ((w && active) ? w[row] : 1.f) : 0.f;
+        const float e2 = s2 * ((w && active) ? w[row] : 1.f);
         const float m = rr.row_max(G);
         float s, t, e[Row::NE];
-        rr.template stats<ENT, true>(G, m, s, t, e);
+        rr.template stats<true, true>(G, m, s, t, e);
         const float logs = logf(s), inv_s = 1.f / s;
         const float H = logs - t * inv_s;  // = -sum p log p
 #pragma unroll
@@ -60,7 +63,7 @@ __global__ void __launch_bounds__(256) softmax_grad_rows_kernel(const float* __r
                 const int idx = rr.index(j, q, G, lig);
                 const float p = e[i] * inv_s;
                 float gq = c * ((idx == a ? 1.f : 0.f) - p);
-                if (ENT) gq += e2 * (-p * (fmaxf(row_logp<CAT>(rr.x[i], m, logs), kNegBig) + H));
+                gq += e2 * (-p * (fmaxf(row_logp<true>(rr.x[i], m, logs), kNegBig) + H));
                 o[q] = gq;
             }
             const int e0 = rr.index(j, 0, G, lig);
@@ -80,14 +83,13 @@ __global__ void __launch_bounds__(256) softmax_grad_rows_kernel(const float* __r
 }
 
 // Staged variant (N <= 32, not 128-bit eligible): see softmax_rows.cuh "Staged rows".
-template <bool ENT, bool CAT>
 __global__ void __launch_bounds__(kStageRows) softmax_grad_rows_staged_kernel(
     const float* __restrict__ logits, const int64_t* __restrict__ action, const float* __restrict__ c1,
     const float* __restrict__ w, const float* __restrict__ g1, const float* __restrict__ g2, float inv_n,
     float* __restrict__ grad, int64_t R, int N, int P, int aligned) {
     extern __shared__ float tile[];
     const float s1 = __ldg(g1);
-    const float s2 = ENT ? __ldg(g2) * inv_n : 0.f;
+    const float s2 = __ldg(g2) * inv_n;
     const int64_t ntiles = (R + kStageRows - 1) / kStageRows;
     for (int64_t tix = blockIdx.x; tix < ntiles; tix += gridDim.x) {
         const int64_t row0 = tix * kStageRows, row = row0 + threadIdx.x;
@@ -97,17 +99,17 @@ __global__ void __launch_bounds__(kStageRows) softmax_grad_rows_staged_kernel(
         if (row < R) {
             float* x = tile + threadIdx.x * P;
             float m, s, t;
-            staged_stats<ENT>(x, N, m, s, t);
+            staged_stats<true>(x, N, m, s, t);
             const float logs = logf(s), inv_s = 1.f / s;
             const float H = logs - t * inv_s;
             const int a = static_cast<int>(action[row]);
             const float c = s1 * c1[row];
-            const float e2 = ENT ? s2 * (w ? w[row] : 1.f) : 0.f;
+            const float e2 = s2 * (w ? w[row] : 1.f);
             for (int k = 0; k < N; ++k) {
                 const float xv = x[k];
                 const float p = exp_term(fmaxf(xv - m, kNegBig)) * inv_s;
                 float gq = c * ((k == a ? 1.f : 0.f) - p);
-                if (ENT) gq += e2 * (-p * (fmaxf(row_logp<CAT>(xv, m, logs), kNegBig) + H));
+                gq += e2 * (-p * (fmaxf(row_logp<true>(xv, m, logs), kNegBig) + H));
                 x[k] = gq;
             }
         }
@@ -117,7 +119,6 @@ __global__ void __launch_bounds__(kStageRows) softmax_grad_rows_staged_kernel(
 }
 
 // N too large for the register-resident path: one warp per row, strided passes over the row.
-template <bool ENT, bool CAT>
 __global__ void __launch_bounds__(256) softmax_grad_rows_loop_kernel(const float* __restrict__ logits,
                                                                       const int64_t* __restrict__ action,
                                                                       const float* __restrict__ c1,
@@ -127,7 +128,7 @@ __global__ void __launch_bounds__(256) softmax_grad_rows_loop_kernel(const float
                                                                       float* __restrict__ grad, int64_t R, int N) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const float s1 = __ldg(g1);
-    const float s2 = ENT ? __ldg(g2) * inv_n : 0.f;
+    const float s2 = __ldg(g2) * inv_n;
     for (int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + warp; row < R; row += static_cast<int64_t>(gridDim.x) * 8) {
         const float* x = logits + row * N;
         float m = -INFINITY;
@@ -138,84 +139,51 @@ __global__ void __launch_bounds__(256) softmax_grad_rows_loop_kernel(const float
         s = warp_sum(s);
         const float logs = logf(s);
         float H = 0.f;
-        if (ENT) {
+        {
             float h = 0.f;
             for (int k = lane; k < N; k += 32) {
-                const float l = fmaxf(row_logp<CAT>(x[k], m, logs), kNegBig);  // -inf logits: 0 * -3e38, not NaN
+                const float l = fmaxf(row_logp<true>(x[k], m, logs), kNegBig);  // -inf logits: 0 * -3e38, not NaN
                 h += exp_term(l) * l;
             }
             H = -warp_sum(h);
         }
         const int a = static_cast<int>(action[row]);
         const float c = s1 * c1[row];
-        const float e2 = ENT ? s2 * (w ? w[row] : 1.f) : 0.f;
+        const float e2 = s2 * (w ? w[row] : 1.f);
         for (int k = lane; k < N; k += 32) {
-            const float l = fmaxf(row_logp<CAT>(x[k], m, logs), kNegBig);  // p = 0 and a finite l for -inf logits
+            const float l = fmaxf(row_logp<true>(x[k], m, logs), kNegBig);  // p = 0 and a finite l for -inf logits
             const float p = exp_term(l);
             float gq = c * ((k == a ? 1.f : 0.f) - p);
-            if (ENT) gq += e2 * (-p * (l + H));
+            gq += e2 * (-p * (l + H));
             grad[row * N + k] = gq;
         }
     }
 }
 
-template <bool ENT, bool CAT>
-static int launch_grad_t(const float* logits, const int64_t* action, const float* c1, const float* w,
-                         const float* g1, const float* g2, float inv_n, float* grad, int64_t R, int N,
-                         cudaStream_t stream) {
-    const RowGeom ge = row_geom(N, logits, grad);
-    if (use_staged_rows(N, ge.width)) {
-        const int P = stage_pitch(N);
-        const unsigned sgrid = rows_grid(R, kStageRows);
-        const int al = aligned16(logits) && aligned16(grad) ? 1 : 0;
-        softmax_grad_rows_staged_kernel<ENT, CAT><<<sgrid, kStageRows, stage_bytes(N, 1), stream>>>(
-            logits, action, c1, w, g1, g2, inv_n, grad, R, N, P, al);
-        count_launch();
-        HPC_LAUNCH_CHECK();
-        return HPC_RLL_OK;
-    }
-    int log2G = 0;
-    while ((1 << log2G) < ge.G) ++log2G;
-    const int rows_per_block = (32 / ge.G) * 8;
-    const unsigned grid = rows_grid(R, ge.kmax == 0 ? 8 : rows_per_block);
-#define HPC_GRAD_LAUNCH(K, V)                                                                                        \
-    do {                                                                                                             \
-        if (ge.G == 1)                                                                                               \
-            softmax_grad_rows_kernel<K, V, ENT, CAT, true><<<grid, 256, 0, stream>>>(logits, action, c1, w, g1, g2,  \
-                                                                                     inv_n, grad, R, N, 1, 0);       \
-        else                                                                                                         \
-            softmax_grad_rows_kernel<K, V, ENT, CAT, false><<<grid, 256, 0, stream>>>(logits, action, c1, w, g1, g2, \
-                                                                                      inv_n, grad, R, N, ge.G,       \
-                                                                                      log2G);                        \
-    } while (0)
-    if (ge.kmax == 0)
-        softmax_grad_rows_loop_kernel<ENT, CAT><<<grid, 256, 0, stream>>>(logits, action, c1, w, g1, g2, inv_n, grad,
-                                                                         R, N);
-    else
-        HPC_ROW_DISPATCH(ge, HPC_GRAD_LAUNCH);
-#undef HPC_GRAD_LAUNCH
-    count_launch();
-    HPC_LAUNCH_CHECK();
-    return HPC_RLL_OK;
-}
+struct GradRows {
+    template <int K, int W, bool G1>
+    static auto reg() { return softmax_grad_rows_kernel<K, W, G1>; }
+    static auto staged() { return softmax_grad_rows_staged_kernel; }
+    static auto loop() { return softmax_grad_rows_loop_kernel; }
+    static constexpr int kStagedTiles = 1;
+};
 
 int launch_softmax_grad_rows(const float* logits, const int64_t* action, const float* c1, const float* w,
                              const float* g1, const float* g2, double inv_n, float* grad, int64_t R, int64_t N,
-                             bool categorical, cudaStream_t stream) {
+                             cudaStream_t stream) {
     if (R <= 0 || N <= 0) return HPC_RLL_OK;
     HPC_REQUIRE(N < (int64_t(1) << 30), "softmax rows: N too large");
-    const float in = static_cast<float>(inv_n);
-    if (g2 != nullptr) {
-        return launch_grad_t<true, true>(logits, action, c1, w, g1, g2, in, grad, R, static_cast<int>(N), stream);
-    }
-    if (categorical)
-        return set_error(HPC_RLL_ENOSUP, "softmax rows: categorical form without entropy term is not instantiated");
-    // The no-entropy gradient (UPGO backward) runs through the ENTROPY instantiation with a zero entropy coefficient
-    // (g2 := g1, inv_n := 0  =>  s2 = 0, every entropy term is 0 * finite): the lighter <.., false, false>
-    // kernel was measured SLOWER on the same traffic: the extra arithmetic spaces the loads and stores of a row out.  Results are bit-identical.
-    return launch_grad_t<true, true>(logits, action, c1, nullptr, g1, g1, 0.f, grad, R, static_cast<int>(N), stream);
+    unsigned grid;
+    if (g2 != nullptr)
+        return launch_rows<GradRows>(&grid, R, N, logits, grad, stream, logits, action, c1, w, g1, g2,
+                                     static_cast<float>(inv_n), grad);
+    // The no-entropy gradient (UPGO backward) runs through the same kernels with a zero entropy coefficient
+    // (g2 := g1, inv_n := 0  =>  s2 = 0, every entropy term is 0 * finite): a lighter kernel without the entropy term was
+    // measured SLOWER on the same traffic: the extra arithmetic spaces the loads and stores of a row out.  Results are
+    // bit-identical.
+    return launch_rows<GradRows>(&grid, R, N, logits, grad, stream, logits, action, c1, static_cast<const float*>(nullptr),
+                                 g1, g1, 0.f, grad);
 }
-
 
 // ---- fixed-order finaliser for several loss terms with different partial counts ---------------------
 __global__ void __launch_bounds__(256) finalize_terms_kernel(const double* __restrict__ partials,

@@ -246,14 +246,183 @@ __device__ __forceinline__ void staged_stats(const float* __restrict__ x, int N,
     t = tt;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Forward row drivers.  V-trace, UPGO and PPO reduce each logits row to (max, log-sum, entropy, the chosen action's
+// log-prob) and differ only in what they do with it.  One driver per row layout walks the rows of the logits tensors
+// l0 and l1 (l1: null when the op has one); the op says what a row is made of and what is done with the result:
+//   kTensors       logits tensors per row (1 or 2), of the same row length N
+//   kEntropy       tensor 0 needs the entropy H (the moment t of the row statistics); H is 0 otherwise
+//   kCat           the log-prob form of row_logp
+//   Scalars scalars(r, ok, lig, args...)          the per-row scalars of row r, `.a` the action (-1 when !ok); lig:
+//                                                 the lane's index in the row's group
+//   emit(row, sc, H, lp0, lp1, args...)           run by one lane per row; lp0 / lp1: the action's log-prob in
+//                                                 tensor 0 / 1
+// args...: the kernel's remaining arguments, passed through as function arguments.  The op struct holds no pointers,
+// only accumulators and per-call constants: a pointer read from a struct member, or values kept in an array, change
+// the register kernels' machine code, so the drivers also name the two tensors' values (x0 / x1, m0 / m1, ...)
+// instead of indexing arrays.
+// ---------------------------------------------------------------------------------------------------
+
+// Register layout: a row in the registers of a group of G lanes, grid-stride over blocks of (32 / G) * 8 rows.
+// G1: one lane per row (G == 1, N == KMAX * WIDTH exactly) known at compile time -- the group loops, the `e0 < N`
+// predicates and the element-index arithmetic of the row helpers fold away (the kernels are bound by instruction issue
+// at small N).  The walk is a macro expanded in the kernel, not a function: behind any call boundary, even a
+// force-inlined one, the 128-bit kernels compile to different machine code.  It expects the kernel's template
+// parameters KMAX, WIDTH, G1 and its arguments R, N_, G_, log2G_ in scope.
+#define HPC_ROWS_FWD_REGS(op, l0, l1, ...)                                                                        \
+    do {                                                                                                          \
+        using Op = decltype(op);                                                                                  \
+        using Row = RowRegs<KMAX, WIDTH>;                                                                         \
+        constexpr bool TWO = Op::kTensors == 2;                                                                   \
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;                                               \
+        const int N = G1 ? KMAX * WIDTH : N_, G = G1 ? 1 : G_, log2G = G1 ? 0 : log2G_;                           \
+        const int lig = G1 ? 0 : (lane & (G - 1)), gw = lane >> log2G;                                            \
+        const int rows_per_warp = 32 >> log2G;                                                                    \
+        const int rows_per_block = rows_per_warp * 8;                                                             \
+        /* software pipeline (small rows only): the next row block's loads are issued before this one is reduced */ \
+        constexpr bool PF = Row::NE <= 8;                                                                         \
+        Row x0, x1, n0, n1;                                                                                       \
+        typename Op::Scalars cur, nxt;                                                                            \
+        /* row index and row pointers advance by increments (no 64-bit multiply per row) */                       \
+        const int64_t stride = static_cast<int64_t>(gridDim.x) * rows_per_block;                                 \
+        int64_t base = static_cast<int64_t>(blockIdx.x) * rows_per_block;                                         \
+        int64_t row = base + warp * rows_per_warp + gw;                                                           \
+        const float* p0 = (l0) + row * N;                                                                         \
+        [[maybe_unused]] const float* p1 = TWO ? static_cast<const float*>(l1) + row * N : nullptr;               \
+        const int64_t pstep = stride * N;                                                                         \
+        x0.load(p0, N, G, lig, row < R);                                                                          \
+        if constexpr (TWO) x1.load(p1, N, G, lig, row < R);                                                       \
+        cur = op.scalars(row, row < R, lig, __VA_ARGS__);                                                         \
+        for (; base < R; base += stride, row += stride) { /* block-uniform trip count */                          \
+            const bool active = row < R;                                                                          \
+            const int64_t nrow = row + stride;                                                                    \
+            p0 += pstep;                                                                                          \
+            if constexpr (TWO) p1 += pstep;                                                                       \
+            if (PF) {                                                                                             \
+                n0.load(p0, N, G, lig, nrow < R);                                                                 \
+                if constexpr (TWO) n1.load(p1, N, G, lig, nrow < R);                                              \
+            }                                                                                                     \
+            if (PF) nxt = op.scalars(nrow, nrow < R, lig, __VA_ARGS__);                                        \
+            const int a = cur.a;                                                                                  \
+            [[maybe_unused]] float m1 = 0.f, s0, t0, s1, t1, none[Row::NE], ls0 = 0.f, ls1 = 0.f, lp1 = 0.f;      \
+            const float m0 = x0.row_max(G);                                                                       \
+            if constexpr (TWO) m1 = x1.row_max(G);                                                                \
+            x0.template stats<Op::kEntropy, false>(G, m0, s0, t0, none);                                          \
+            if constexpr (TWO) x1.template stats<false, false>(G, m1, s1, t1, none);                              \
+            if constexpr (Op::kEntropy) ls0 = logf(s0);                                                           \
+            if constexpr (TWO) ls1 = logf(s1);                                                                    \
+            const float H = Op::kEntropy ? ls0 - t0 / s0 : 0.f;                                                   \
+            /* exactly one lane of the group holds the action's logit */                                          \
+            /* (log s after the selection when nothing else needs it: the order the UPGO kernels were tuned in) */ \
+            const float lp0 = row_logp<Op::kCat>(group_sum(x0.select(a, G, lig), G), m0, Op::kEntropy ? ls0 : logf(s0)); \
+            if constexpr (TWO) lp1 = row_logp<Op::kCat>(group_sum(x1.select(a, G, lig), G), m1, ls1);             \
+            if (active && lig == 0) op.emit(row, cur, H, lp0, lp1, __VA_ARGS__);                                  \
+            if (PF) {                                                                                             \
+                x0 = n0;                                                                                          \
+                if constexpr (TWO) x1 = n1;                                                                       \
+            } else {                                                                                              \
+                x0.load(p0, N, G, lig, nrow < R);                                                                 \
+                if constexpr (TWO) x1.load(p1, N, G, lig, nrow < R);                                              \
+            }                                                                                                     \
+            if (PF) cur = nxt;                                                                                    \
+            else cur = op.scalars(nrow, nrow < R, lig, __VA_ARGS__);                                              \
+        }                                                                                                         \
+    } while (0)
+
+// Staged layout (N <= 32, not 128-bit eligible, see "Staged rows" above): kTensors tiles of kStageRows rows in dynamic
+// shared memory, one thread per row.
+template <class Op, class... A>
+__device__ __forceinline__ void rows_fwd_staged(Op& op, int64_t R, int N, int P, int aligned, const float* l0,
+                                                const float* l1, A... args) {
+    constexpr bool TWO = Op::kTensors == 2;
+    extern __shared__ float tiles[];
+    float* tile0 = tiles;
+    float* tile1 = tiles + kStageRows * P;
+    const int64_t ntiles = (R + kStageRows - 1) / kStageRows;
+    for (int64_t tix = blockIdx.x; tix < ntiles; tix += gridDim.x) {
+        const int64_t row0 = tix * kStageRows, row = row0 + threadIdx.x;
+        __syncthreads();  // every thread is done with the previous tiles
+        stage_rows(l0, R, N, P, row0, tile0, aligned != 0);
+        if constexpr (TWO) stage_rows(l1, R, N, P, row0, tile1, aligned != 0);
+        __syncthreads();
+        if (row < R) {
+            const float* x0 = tile0 + threadIdx.x * P;
+            const float* x1 = tile1 + threadIdx.x * P;
+            float m0, s0, t0, m1 = 0.f, s1 = 0.f, t1, ls1 = 0.f, lp1 = 0.f;
+            staged_stats<Op::kEntropy>(x0, N, m0, s0, t0);
+            if constexpr (TWO) staged_stats<false>(x1, N, m1, s1, t1);
+            const float ls0 = logf(s0);
+            if constexpr (TWO) ls1 = logf(s1);
+            const float H = Op::kEntropy ? ls0 - t0 / s0 : 0.f;
+            const typename Op::Scalars sc = op.scalars(row, true, 0, args...);
+            const float lp0 = row_logp<Op::kCat>(x0[sc.a], m0, ls0);
+            if constexpr (TWO) lp1 = row_logp<Op::kCat>(x1[sc.a], m1, ls1);
+            op.emit(row, sc, H, lp0, lp1, args...);
+        }
+    }
+}
+
+// Looping layout (N too large for registers): one warp per row, strided passes over the row.
+template <class Op, class... A>
+__device__ __forceinline__ void rows_fwd_loop(Op& op, int64_t R, int N, const float* l0, const float* l1, A... args) {
+    constexpr bool TWO = Op::kTensors == 2;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + warp; row < R; row += static_cast<int64_t>(gridDim.x) * 8) {
+        const float* x0 = l0 + row * N;
+        const float* x1 = l1 + row * N;
+        float m0 = -INFINITY, m1 = -INFINITY;
+        for (int k = lane; k < N; k += 32) {
+            m0 = fmaxf(m0, x0[k]);
+            if constexpr (TWO) m1 = fmaxf(m1, x1[k]);
+        }
+        m0 = warp_max(m0);
+        if constexpr (TWO) m1 = warp_max(m1);
+        float s0 = 0.f, s1 = 0.f;
+        for (int k = lane; k < N; k += 32) {
+            s0 += exp_term(x0[k] - m0);
+            if constexpr (TWO) s1 += exp_term(x1[k] - m1);
+        }
+        s0 = warp_sum(s0);
+        if constexpr (TWO) s1 = warp_sum(s1);
+        float ls1 = 0.f, lp1 = 0.f, H = 0.f;
+        const float ls0 = logf(s0);
+        if constexpr (TWO) ls1 = logf(s1);
+        if constexpr (Op::kEntropy) {
+            float h = 0.f;
+            for (int k = lane; k < N; k += 32) {
+                const float lp = fmaxf(row_logp<Op::kCat>(x0[k], m0, ls0), kNegBig);  // -inf logits: 0 * -3e38, not NaN
+                h += exp_term(lp) * lp;
+            }
+            H = -warp_sum(h);
+        }
+        if (lane == 0) {
+            const typename Op::Scalars sc = op.scalars(row, true, 0, args...);
+            const float lp0 = row_logp<Op::kCat>(x0[sc.a], m0, ls0);
+            if constexpr (TWO) lp1 = row_logp<Op::kCat>(x1[sc.a], m1, ls1);
+            op.emit(row, sc, H, lp0, lp1, args...);
+        }
+    }
+}
+
+// one fp64 partial per CTA and term: partials[k * gridDim.x + blockIdx.x]
+template <int K>
+__device__ __forceinline__ void flush_partials(double (&acc)[K], double* __restrict__ partials) {
+    __shared__ double red[K * 32];
+    block_sum<K>(acc, red);
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) partials[static_cast<size_t>(k) * gridDim.x + blockIdx.x] = acc[k];
+    }
+}
+
 #endif  // __CUDACC__
 
 // ---- shared backward: grad[r,k] = (g1*c1[r])*(1[k=a_r]-p_k) + (g2*w_r*inv_n)*(-p_k(logp_k+H)) ----------
 // g1, g2: device scalars (upstream gradients); g2 == nullptr skips the entropy term; w == nullptr -> 1.
-// categorical selects the log-prob normalisation (see row_logp).
+// Categorical log-probs (see row_logp).
 int launch_softmax_grad_rows(const float* logits, const int64_t* action, const float* c1, const float* w,
                              const float* g1, const float* g2, double inv_n, float* grad, int64_t R, int64_t N,
-                             bool categorical, cudaStream_t stream);
+                             cudaStream_t stream);
 
 // grid size for a row-streaming kernel: enough CTAs to fill the machine, grid-stride over row blocks
 inline unsigned rows_grid(int64_t R, int rows_per_block) {
@@ -272,23 +441,62 @@ struct FinSpec {
 };
 int launch_finalize_terms(const double* partials, const FinSpec& spec, int nterms, float* out, cudaStream_t stream);
 
-// dispatch helper: expands to the KMAX/WIDTH instantiation selected by a RowGeom
-#define HPC_ROW_DISPATCH_W(ge, LAUNCH, WD)      \
-    switch ((ge).kmax) {                        \
-        case 1: LAUNCH(1, WD); break;           \
-        case 2: LAUNCH(2, WD); break;           \
-        case 3: LAUNCH(3, WD); break;           \
-        case 4: LAUNCH(4, WD); break;           \
-        case 5: LAUNCH(5, WD); break;           \
-        case 6: LAUNCH(6, WD); break;           \
-        case 7: LAUNCH(7, WD); break;           \
-        default: LAUNCH(8, WD); break;          \
+// The register layouts (WIDTH, G1, KMAX) row_geom and use_staged_rows can select, and the only ones built: with G == 1
+// every KMAX up to the lane's chunk cap (4 float4, 8 narrower); G > 1 only when the row has more chunks than that cap,
+// so more than half of it per lane; width 1 with 9 <= N <= 32 is staged.  tests/test_row_layouts_cpu.py checks this
+// table against the built library and the dispatch mirror of tests/row_paths.py.
+#define HPC_ROW_LAYOUTS(X)                                                                               \
+    X(4, true, 1) X(4, true, 2) X(4, true, 3) X(4, true, 4)                                              \
+    X(2, true, 1) X(2, true, 2) X(2, true, 3) X(2, true, 4) X(2, true, 5) X(2, true, 6) X(2, true, 7) X(2, true, 8) \
+    X(1, true, 1) X(1, true, 2) X(1, true, 3) X(1, true, 4) X(1, true, 5) X(1, true, 6) X(1, true, 7) X(1, true, 8) \
+    X(4, false, 3) X(4, false, 4) X(4, false, 5) X(4, false, 6) X(4, false, 7) X(4, false, 8)            \
+    X(2, false, 5) X(2, false, 6) X(2, false, 7) X(2, false, 8)                                          \
+    X(1, false, 5) X(1, false, 6) X(1, false, 7) X(1, false, 8)
+
+constexpr int row_layout_key(int width, bool g1, int kmax) { return (width * 2 + (g1 ? 1 : 0)) * 16 + kmax; }
+
+#ifdef __CUDACC__
+// Launches the row kernel of one family that row_geom / use_staged_rows pick for rows of N floats.  p0, p1: the row
+// tensors whose alignment decides the layout (p1 may be null).  Rows::reg<KMAX, WIDTH, G1>(), Rows::staged() and
+// Rows::loop() return the family's kernels, which take args... followed by (R, N, G, log2G), (R, N, pitch, aligned)
+// and (R, N); the staged kernel holds Rows::kStagedTiles tiles.  *grid: the CTA count (the caller's partial count).
+template <class Rows, class... Args>
+int launch_rows(unsigned* grid, int64_t R, int64_t N, const void* p0, const void* p1, cudaStream_t stream,
+                Args... args) {
+    const RowGeom ge = row_geom(N, p0, p1);
+    const int n = static_cast<int>(N);
+    if (use_staged_rows(N, ge.width)) {
+        const int max_bytes = static_cast<int>(stage_bytes(32, Rows::kStagedTiles));  // largest pitch (N=32 -> 33)
+        if (max_bytes > 48 * 1024) {
+            static SmemOptIn opt;
+            if (int rc = opt.ensure(Rows::staged(), max_bytes)) return rc;
+        }
+        *grid = rows_grid(R, kStageRows);
+        Rows::staged()<<<*grid, kStageRows, stage_bytes(n, Rows::kStagedTiles), stream>>>(
+            args..., R, n, stage_pitch(n), aligned16(p0) && (!p1 || aligned16(p1)) ? 1 : 0);
+    } else if (ge.kmax == 0) {
+        *grid = rows_grid(R, 8);
+        Rows::loop()<<<*grid, 256, 0, stream>>>(args..., R, n);
+    } else {
+        int log2G = 0;
+        while ((1 << log2G) < ge.G) ++log2G;
+        *grid = rows_grid(R, (32 / ge.G) * 8);
+        decltype(Rows::template reg<1, 1, true>()) kernel;
+        switch (row_layout_key(ge.width, ge.G == 1, ge.kmax)) {
+#define HPC_ROW_CASE(W, G1, K) \
+    case row_layout_key(W, G1, K): kernel = Rows::template reg<K, W, G1>(); break;
+            HPC_ROW_LAYOUTS(HPC_ROW_CASE)
+#undef HPC_ROW_CASE
+            default:
+                return set_error(HPC_RLL_ENOSUP, "row kernels: no register layout for width %d, G %d, kmax %d", ge.width,
+                                 ge.G, ge.kmax);
+        }
+        kernel<<<*grid, 256, 0, stream>>>(args..., R, n, ge.G, log2G);
     }
-#define HPC_ROW_DISPATCH(ge, LAUNCH)                                 \
-    do {                                                             \
-        if ((ge).width == 4) { HPC_ROW_DISPATCH_W(ge, LAUNCH, 4) }   \
-        else if ((ge).width == 2) { HPC_ROW_DISPATCH_W(ge, LAUNCH, 2) } \
-        else { HPC_ROW_DISPATCH_W(ge, LAUNCH, 1) }                   \
-    } while (0)
+    count_launch();
+    HPC_LAUNCH_CHECK();
+    return HPC_RLL_OK;
+}
+#endif  // __CUDACC__
 
 }  // namespace hpcrll

@@ -18,88 +18,54 @@
 
 namespace hpcrll {
 
-// G1: one lane per row known at compile time (G == 1, N == KMAX * WIDTH): see ppo_rows_fwd
-template <int KMAX, int WIDTH, bool G1 = false>
+// one logits row -> the log-softmax of the chosen action (`metric`); args: (action, metric)
+struct UpgoRowOp {
+    static constexpr int kTensors = 1;
+    static constexpr bool kEntropy = false, kCat = false;
+    struct Scalars {
+        int a;
+    };
+    __device__ __forceinline__ Scalars scalars(int64_t r, bool ok, int, const int64_t* __restrict__ action,
+                                               float*) const {
+        return {ok ? static_cast<int>(action[r]) : -1};
+    }
+    __device__ __forceinline__ void emit(int64_t row, const Scalars&, float, float lp0, float, const int64_t*,
+                                         float* __restrict__ metric) const {
+        metric[row] = lp0;
+    }
+};
+
+template <int KMAX, int WIDTH, bool G1>
 __global__ void __launch_bounds__(256) upgo_rows_fwd(const float* __restrict__ logits,
                                                       const int64_t* __restrict__ action,
                                                       float* __restrict__ metric, int64_t R, int N_, int G_,
                                                       int log2G_) {
-    using Row = RowRegs<KMAX, WIDTH>;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int N = G1 ? KMAX * WIDTH : N_, G = G1 ? 1 : G_, log2G = G1 ? 0 : log2G_;
-    const int lig = G1 ? 0 : (lane & (G - 1)), gw = lane >> log2G;
-    const int rows_per_warp = 32 >> log2G;
-    const int rows_per_block = rows_per_warp * 8;
-    constexpr bool PF = Row::NE <= 8;  // software pipeline (see softmax_rows.cu)
-    Row rr, nx;
-    int a, na = -1;
-    // row index and row pointer advance by increments (no 64-bit multiply per row)
-    const int64_t stride = static_cast<int64_t>(gridDim.x) * rows_per_block;
-    int64_t base = static_cast<int64_t>(blockIdx.x) * rows_per_block;
-    int64_t row = base + warp * rows_per_warp + gw;
-    const float* pl = logits + row * N;
-    const int64_t pstep = stride * N;
-    rr.load(pl, N, G, lig, row < R);
-    a = row < R ? static_cast<int>(action[row]) : -1;
-    for (; base < R; base += stride, row += stride) {  // block-uniform trip count
-        const bool active = row < R;
-        const int64_t nrow = row + stride;
-        pl += pstep;
-        if (PF) {
-            nx.load(pl, N, G, lig, nrow < R);
-            na = nrow < R ? static_cast<int>(action[nrow]) : -1;
-        }
-        const float m = rr.row_max(G);
-        float s, t, none[Row::NE];
-        rr.template stats<false, false>(G, m, s, t, none);
-        const float sel = row_logp<false>(group_sum(rr.select(a, G, lig), G), m, logf(s));
-        if (active && lig == 0) metric[row] = sel;
-        if (PF) {
-            rr = nx;
-            a = na;
-        } else {
-            rr.load(pl, N, G, lig, nrow < R);
-            a = nrow < R ? static_cast<int>(action[nrow]) : -1;
-        }
-    }
+    UpgoRowOp op;
+    HPC_ROWS_FWD_REGS(op, logits, nullptr, action, metric);
 }
 
-// staged variant (N <= 32, not 128-bit eligible): see softmax_rows.cuh "Staged rows"
 __global__ void __launch_bounds__(kStageRows) upgo_rows_fwd_staged(const float* __restrict__ logits,
                                                                     const int64_t* __restrict__ action,
                                                                     float* __restrict__ metric, int64_t R, int N, int P,
                                                                     int aligned) {
-    extern __shared__ float tile[];
-    const int64_t ntiles = (R + kStageRows - 1) / kStageRows;
-    for (int64_t tix = blockIdx.x; tix < ntiles; tix += gridDim.x) {
-        const int64_t row0 = tix * kStageRows, row = row0 + threadIdx.x;
-        __syncthreads();
-        stage_rows(logits, R, N, P, row0, tile, aligned != 0);
-        __syncthreads();
-        if (row < R) {
-            const float* x = tile + threadIdx.x * P;
-            float m, s, t;
-            staged_stats<false>(x, N, m, s, t);
-            metric[row] = row_logp<false>(x[action[row]], m, logf(s));
-        }
-    }
+    UpgoRowOp op;
+    rows_fwd_staged(op, R, N, P, aligned, logits, nullptr, action, metric);
 }
 
 __global__ void __launch_bounds__(256) upgo_rows_fwd_loop(const float* __restrict__ logits,
                                                            const int64_t* __restrict__ action,
                                                            float* __restrict__ metric, int64_t R, int N) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + warp; row < R; row += static_cast<int64_t>(gridDim.x) * 8) {
-        const float* x = logits + row * N;
-        float m = -INFINITY;
-        for (int k = lane; k < N; k += 32) m = fmaxf(m, x[k]);
-        m = warp_max(m);
-        float s = 0.f;
-        for (int k = lane; k < N; k += 32) s += exp_term(x[k] - m);
-        s = warp_sum(s);
-        if (lane == 0) metric[row] = row_logp<false>(x[action[row]], m, logf(s));
-    }
+    UpgoRowOp op;
+    rows_fwd_loop(op, R, N, logits, nullptr, action, metric);
 }
+
+struct UpgoRows {
+    template <int K, int W, bool G1>
+    static auto reg() { return upgo_rows_fwd<K, W, G1>; }
+    static auto staged() { return upgo_rows_fwd_staged; }
+    static auto loop() { return upgo_rows_fwd_loop; }
+    static constexpr int kStagedTiles = 1;
+};
 
 struct UpgoBody {
     float ret, v1, v2, r1, neg_inv_n;
@@ -280,29 +246,9 @@ int hpc_rll_upgo_forward(const float* target_output, const float* rhos, const in
     double* partials = reinterpret_cast<double*>(ws + align_up_(R * 4, 256));
     const double inv_n = 1.0 / (static_cast<double>(T) * static_cast<double>(global_B));
 
-    const RowGeom ge = row_geom(N, target_output);
-    int log2G = 0;
-    while ((1 << log2G) < ge.G) ++log2G;
-    const bool staged = use_staged_rows(N, ge.width);
-    const unsigned grid1 = rows_grid(R, staged ? kStageRows : (ge.kmax == 0 ? 8 : (32 / ge.G) * 8));
-    const int n = static_cast<int>(N);
-#define HPC_UP_ROWS(K, V)                                                                                       \
-    do {                                                                                                        \
-        if (ge.G == 1)                                                                                          \
-            upgo_rows_fwd<K, V, true><<<grid1, 256, 0, stream>>>(target_output, action, metric, R, n, 1, 0);    \
-        else                                                                                                    \
-            upgo_rows_fwd<K, V, false><<<grid1, 256, 0, stream>>>(target_output, action, metric, R, n, ge.G,    \
-                                                                  log2G);                                       \
-    } while (0)
-    if (staged)
-        upgo_rows_fwd_staged<<<grid1, kStageRows, stage_bytes(n, 1), stream>>>(target_output, action, metric, R, n,
-                                                                               stage_pitch(n),
-                                                                               aligned16(target_output) ? 1 : 0);
-    else if (ge.kmax == 0) upgo_rows_fwd_loop<<<grid1, 256, 0, stream>>>(target_output, action, metric, R, n);
-    else HPC_ROW_DISPATCH(ge, HPC_UP_ROWS);
-#undef HPC_UP_ROWS
-    count_launch();
-    HPC_LAUNCH_CHECK();
+    unsigned grid1;
+    if (int rc1 = launch_rows<UpgoRows>(&grid1, R, N, target_output, nullptr, stream, target_output, action, metric))
+        return rc1;
 
     const float nin = static_cast<float>(-inv_n);
     const bool tma = tma_ok_2d(bootstrap_values, B, B) && tma_ok_2d(rewards, B, B) && tma_ok_2d(rhos, B, B);
@@ -349,7 +295,7 @@ int hpc_rll_upgo_backward(const float* grad_loss, const float* target_output, co
     HPC_REQUIRE(T > 0 && B > 0 && N > 0, "upgo_backward: sizes must be positive");
     HPC_REQUIRE(grad_loss && target_output && action && coef && grad_target_output, "upgo_backward: null pointer");
     return launch_softmax_grad_rows(target_output, action, coef, nullptr, grad_loss, nullptr, 0.0,
-                                    grad_target_output, T * B, N, false, as_stream(stream_));
+                                    grad_target_output, T * B, N, as_stream(stream_));
 }
 
 }  // extern "C"

@@ -26,76 +26,40 @@ namespace hpcrll {
 // ------------------------------------------------------------------------------------------------
 // forward stage 1: rows
 // ------------------------------------------------------------------------------------------------
-// G1: one lane per row known at compile time (G == 1, N == KMAX * WIDTH): see ppo_rows_fwd
-template <int KMAX, int WIDTH, bool G1 = false>
+// one (target, behaviour) row pair -> IS and the target's log-prob of the chosen action, and the entropy partial;
+// args: (action, weight, is_out, logp_out)
+struct VtraceRowOp {
+    static constexpr int kTensors = 2;
+    static constexpr bool kEntropy = true, kCat = true;
+    struct Scalars {
+        int a;
+    };
+    double acc[1] = {0.0};
+    __device__ __forceinline__ Scalars scalars(int64_t r, bool ok, int, const int64_t* __restrict__ action,
+                                               const float*, float*, float*) const {
+        return {ok ? static_cast<int>(action[r]) : -1};
+    }
+    __device__ __forceinline__ void emit(int64_t row, const Scalars&, float H, float lp0, float lp1, const int64_t*,
+                                         const float* __restrict__ weight, float* __restrict__ is_out,
+                                         float* __restrict__ logp_out) {
+        is_out[row] = expf(lp0 - lp1);
+        logp_out[row] = lp0;
+        acc[0] += static_cast<double>(H * (weight ? weight[row] : 1.f));
+    }
+};
+
+template <int KMAX, int WIDTH, bool G1>
 __global__ void __launch_bounds__(256) vtrace_rows_fwd(const float* __restrict__ target,
                                                         const float* __restrict__ behaviour,
                                                         const int64_t* __restrict__ action,
                                                         const float* __restrict__ weight, float* __restrict__ is_out,
                                                         float* __restrict__ logp_out, double* __restrict__ partials,
                                                         int64_t R, int N_, int G_, int log2G_) {
-    using Row = RowRegs<KMAX, WIDTH>;
-    __shared__ double red[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int N = G1 ? KMAX * WIDTH : N_, G = G1 ? 1 : G_, log2G = G1 ? 0 : log2G_;
-    const int lig = G1 ? 0 : (lane & (G - 1)), gw = lane >> log2G;
-    const int rows_per_warp = 32 >> log2G;
-    const int rows_per_block = rows_per_warp * 8;
-    double ent_acc = 0.0;
-    // software pipeline: next row block's loads are issued before this block is reduced
-    constexpr bool PF = Row::NE <= 8;
-    Row rt, rbh, nt, nb;
-    int a, na = -1;
-    // row index and row pointers advance by increments (no 64-bit multiply per row)
-    const int64_t stride = static_cast<int64_t>(gridDim.x) * rows_per_block;
-    int64_t base = static_cast<int64_t>(blockIdx.x) * rows_per_block;
-    int64_t row = base + warp * rows_per_warp + gw;
-    const float* pt = target + row * N;
-    const float* pb = behaviour + row * N;
-    const int64_t pstep = stride * N;
-    rt.load(pt, N, G, lig, row < R);
-    rbh.load(pb, N, G, lig, row < R);
-    a = row < R ? static_cast<int>(action[row]) : -1;
-    for (; base < R; base += stride, row += stride) {  // block-uniform trip count
-        const bool active = row < R;
-        const int64_t nrow = row + stride;
-        pt += pstep;
-        pb += pstep;
-        if (PF) {
-            nt.load(pt, N, G, lig, nrow < R);
-            nb.load(pb, N, G, lig, nrow < R);
-            na = nrow < R ? static_cast<int>(action[nrow]) : -1;
-        }
-        const float mt = rt.row_max(G), mb = rbh.row_max(G);
-        float st, tt, sb, tb, none[Row::NE];
-        rt.template stats<true, false>(G, mt, st, tt, none);
-        rbh.template stats<false, false>(G, mb, sb, tb, none);
-        const float lst = logf(st), lsb = logf(sb);
-        const float H = lst - tt / st;  // entropy of the target policy
-        // exactly one lane of the group holds the action's logit
-        const float selt = row_logp<true>(group_sum(rt.select(a, G, lig), G), mt, lst);
-        const float selb = row_logp<true>(group_sum(rbh.select(a, G, lig), G), mb, lsb);
-        if (active && lig == 0) {
-            is_out[row] = expf(selt - selb);
-            logp_out[row] = selt;
-            ent_acc += static_cast<double>(H * (weight ? weight[row] : 1.f));
-        }
-        if (PF) {
-            rt = nt;
-            rbh = nb;
-            a = na;
-        } else {
-            rt.load(pt, N, G, lig, nrow < R);
-            rbh.load(pb, N, G, lig, nrow < R);
-            a = nrow < R ? static_cast<int>(action[nrow]) : -1;
-        }
-    }
-    double v[1] = {ent_acc};
-    block_sum<1>(v, red);
-    if (threadIdx.x == 0) partials[blockIdx.x] = v[0];
+    VtraceRowOp op;
+    HPC_ROWS_FWD_REGS(op, target, behaviour, action, weight, is_out, logp_out);
+    flush_partials(op.acc, partials);
 }
 
-// staged variant (N <= 32, not 128-bit eligible): see softmax_rows.cuh "Staged rows"
 __global__ void __launch_bounds__(kStageRows) vtrace_rows_fwd_staged(const float* __restrict__ target,
                                                                       const float* __restrict__ behaviour,
                                                                       const int64_t* __restrict__ action,
@@ -104,84 +68,29 @@ __global__ void __launch_bounds__(kStageRows) vtrace_rows_fwd_staged(const float
                                                                       float* __restrict__ logp_out,
                                                                       double* __restrict__ partials, int64_t R, int N,
                                                                       int P, int aligned) {
-    extern __shared__ float tiles[];
-    __shared__ double red[32];
-    float* tt = tiles;
-    float* tb = tiles + kStageRows * P;
-    double ent_acc = 0.0;
-    const int64_t ntiles = (R + kStageRows - 1) / kStageRows;
-    for (int64_t tix = blockIdx.x; tix < ntiles; tix += gridDim.x) {
-        const int64_t row0 = tix * kStageRows, row = row0 + threadIdx.x;
-        __syncthreads();
-        stage_rows(target, R, N, P, row0, tt, aligned != 0);
-        stage_rows(behaviour, R, N, P, row0, tb, aligned != 0);
-        __syncthreads();
-        if (row < R) {
-            const float* xt = tt + threadIdx.x * P;
-            const float* xb = tb + threadIdx.x * P;
-            float mt, st, t1, mb, sb, t2;
-            staged_stats<true>(xt, N, mt, st, t1);
-            staged_stats<false>(xb, N, mb, sb, t2);
-            const float lst = logf(st), lsb = logf(sb);
-            const float H = lst - t1 / st;
-            const int a = static_cast<int>(action[row]);
-            const float selt = row_logp<true>(xt[a], mt, lst), selb = row_logp<true>(xb[a], mb, lsb);
-            is_out[row] = expf(selt - selb);
-            logp_out[row] = selt;
-            ent_acc += static_cast<double>(H * (weight ? weight[row] : 1.f));
-        }
-    }
-    double v[1] = {ent_acc};
-    block_sum<1>(v, red);
-    if (threadIdx.x == 0) partials[blockIdx.x] = v[0];
+    VtraceRowOp op;
+    rows_fwd_staged(op, R, N, P, aligned, target, behaviour, action, weight, is_out, logp_out);
+    flush_partials(op.acc, partials);
 }
 
-// N too large for registers: one warp per row, strided passes
 __global__ void __launch_bounds__(256) vtrace_rows_fwd_loop(const float* __restrict__ target,
                                                              const float* __restrict__ behaviour,
                                                              const int64_t* __restrict__ action,
                                                              const float* __restrict__ weight,
                                                              float* __restrict__ is_out, float* __restrict__ logp_out,
                                                              double* __restrict__ partials, int64_t R, int N) {
-    __shared__ double red[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    double ent_acc = 0.0;
-    for (int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + warp; row < R; row += static_cast<int64_t>(gridDim.x) * 8) {
-        const float* xt = target + row * N;
-        const float* xb = behaviour + row * N;
-        float mt = -INFINITY, mb = -INFINITY;
-        for (int k = lane; k < N; k += 32) {
-            mt = fmaxf(mt, xt[k]);
-            mb = fmaxf(mb, xb[k]);
-        }
-        mt = warp_max(mt);
-        mb = warp_max(mb);
-        float st = 0.f, sb = 0.f;
-        for (int k = lane; k < N; k += 32) {
-            st += exp_term(xt[k] - mt);
-            sb += exp_term(xb[k] - mb);
-        }
-        st = warp_sum(st);
-        sb = warp_sum(sb);
-        const float lst = logf(st), lsb = logf(sb);
-        float h = 0.f;
-        for (int k = lane; k < N; k += 32) {
-            const float lp = fmaxf(row_logp<true>(xt[k], mt, lst), kNegBig);  // -inf logits: 0 * -3e38, not NaN
-            h += exp_term(lp) * lp;
-        }
-        const float H = -warp_sum(h);
-        if (lane == 0) {
-            const int a = static_cast<int>(action[row]);
-            const float selt = row_logp<true>(xt[a], mt, lst), selb = row_logp<true>(xb[a], mb, lsb);
-            is_out[row] = expf(selt - selb);
-            logp_out[row] = selt;
-            ent_acc += static_cast<double>(H * (weight ? weight[row] : 1.f));
-        }
-    }
-    double v[1] = {ent_acc};
-    block_sum<1>(v, red);
-    if (threadIdx.x == 0) partials[blockIdx.x] = v[0];
+    VtraceRowOp op;
+    rows_fwd_loop(op, R, N, target, behaviour, action, weight, is_out, logp_out);
+    flush_partials(op.acc, partials);
 }
+
+struct VtraceRows {
+    template <int K, int W, bool G1>
+    static auto reg() { return vtrace_rows_fwd<K, W, G1>; }
+    static auto staged() { return vtrace_rows_fwd_staged; }
+    static auto loop() { return vtrace_rows_fwd_loop; }
+    static constexpr int kStagedTiles = 2;
+};
 
 // ------------------------------------------------------------------------------------------------
 // forward stage 2: scan
@@ -436,36 +345,10 @@ int hpc_rll_vtrace_forward(const float* target_output, const float* behaviour_ou
     const double inv_n = 1.0 / (static_cast<double>(T) * static_cast<double>(global_B));
 
     // ---- stage 1: rows ----
-    const RowGeom ge = row_geom(N, target_output, behaviour_output);
-    int log2G = 0;
-    while ((1 << log2G) < ge.G) ++log2G;
-    const int rows_per_block = (32 / ge.G) * 8;
-    const bool staged = use_staged_rows(N, ge.width);
-    const unsigned grid1 = rows_grid(R, staged ? kStageRows : (ge.kmax == 0 ? 8 : rows_per_block));
-    const int n = static_cast<int>(N);
-#define HPC_VT_ROWS(K, V)                                                                                             \
-    do {                                                                                                              \
-        if (ge.G == 1)                                                                                                \
-            vtrace_rows_fwd<K, V, true><<<grid1, 256, 0, stream>>>(target_output, behaviour_output, action, weight,   \
-                                                                   is_buf, logp_buf, partials, R, n, 1, 0);           \
-        else                                                                                                          \
-            vtrace_rows_fwd<K, V, false><<<grid1, 256, 0, stream>>>(target_output, behaviour_output, action, weight,  \
-                                                                    is_buf, logp_buf, partials, R, n, ge.G, log2G);   \
-    } while (0)
-    if (staged) {
-        static SmemOptIn opt;
-        if (int rc0 = opt.ensure(vtrace_rows_fwd_staged, static_cast<int>(stage_bytes(32, 2)))) return rc0;  // largest pitch (N=32 -> 33)
-        vtrace_rows_fwd_staged<<<grid1, kStageRows, stage_bytes(n, 2), stream>>>(
-            target_output, behaviour_output, action, weight, is_buf, logp_buf, partials, R, n, stage_pitch(n),
-            aligned16(target_output) && aligned16(behaviour_output) ? 1 : 0);
-    } else if (ge.kmax == 0)
-        vtrace_rows_fwd_loop<<<grid1, 256, 0, stream>>>(target_output, behaviour_output, action, weight, is_buf,
-                                                        logp_buf, partials, R, n);
-    else
-        HPC_ROW_DISPATCH(ge, HPC_VT_ROWS);
-#undef HPC_VT_ROWS
-    count_launch();
-    HPC_LAUNCH_CHECK();
+    unsigned grid1;
+    if (int rc1 = launch_rows<VtraceRows>(&grid1, R, N, target_output, behaviour_output, stream, target_output,
+                                          behaviour_output, action, weight, is_buf, logp_buf, partials))
+        return rc1;
 
     // ---- stage 2: scan ----
     const float g = static_cast<float>(gamma), f = static_cast<float>(gamma * lambda);
@@ -552,7 +435,7 @@ int hpc_rll_vtrace_backward(const float* grad_policy_loss, const float* grad_val
     if (global_B <= 0) global_B = B;
     const double inv_n = 1.0 / (static_cast<double>(T) * static_cast<double>(global_B));
     int rc = launch_softmax_grad_rows(target_output, action, pg_coef, weight, grad_policy_loss, grad_entropy_loss,
-                                      inv_n, grad_target_output, T * B, N, true, stream);
+                                      inv_n, grad_target_output, T * B, N, stream);
     if (rc) return rc;
     return launch_scale_copy(gv_buf, grad_value_loss, grad_value, T * B, B, stream);
 }

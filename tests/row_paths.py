@@ -76,6 +76,21 @@ def row_path(op, direction, N, off, R, sms):
     return Path(kind, rpb, grid, max(1, (last + stride - 1) // stride))
 
 
+def row_layouts():
+    """every row kernel the dispatch can select: (family, width, G1, kmax) for a register layout (G1: one lane per row),
+    (family, "staged") and (family, "loop"); family: the op of a forward, "grad" for the backward all three share.  N runs
+    past the three looping thresholds (257, 514, 1028) at every float offset of the logits"""
+    out = set()
+    for op in OPS:
+        for direction in DIRECTIONS:
+            family = op if direction == "fwd" else "grad"
+            for N in range(1, 1101):
+                for off in range(4):
+                    kind = row_path(op, direction, N, off, 1000, 132).kind
+                    out.add((family, kind[1], kind[2] == 1, kind[3]) if kind[0] == "reg" else (family, kind[0]))
+    return out
+
+
 def wrap_rows(N, off, sms):
     """a ragged row count at which every CTA of the (N, off) path makes at least two grid-stride passes"""
     p = row_path("upgo", "fwd", N, off, 1, sms)
