@@ -75,9 +75,11 @@ int make_tmap_2d(CUtensorMap* out, const float* base, int64_t rows, int64_t cols
 int make_tmap_2d_u8(CUtensorMap* out, const uint8_t* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
                     int box_cols);
 
-// Opt a kernel into > 48 KB dynamic shared memory.  The attribute is per context and holds the LARGEST byte count
-// granted so far per device: kernels whose dynamic size varies at run time (n_atom / tau dependent, nstep.cu) are
-// re-opted whenever a call needs more than any earlier one (ADVICE r1: a first call at ~50 KB used to pin the limit).
+// Opt a kernel into more dynamic shared memory than it may use by default: 48 KB minus its static shared memory (a
+// launch above that fails).  The first opt-in also sets the kernel's carveout to the largest shared-memory share.  The
+// attribute is per context and holds the LARGEST byte count granted so far per device: kernels whose dynamic size
+// varies at run time (n_atom / tau dependent, nstep.cu) are re-opted whenever a call needs more than any earlier one
+// (ADVICE r1: a first call at ~50 KB used to pin the limit).
 struct SmemOptIn {
     int granted[64] = {};
     template <typename K>

@@ -101,9 +101,11 @@ def softmax(x):
     return (e / e.sum(-1, keepdims=True)).astype(np.float32)
 
 
+# n_atom 1536: exactly 48 KB of dynamic shared memory, over the limit with the warp kernel's static shared memory
 @pytest.mark.parametrize("T,B,N,n_atom,use_w,vr", [(128, 128, 128, 51, False, (-10.0, 10.0)), (5, 1000, 4, 51, True, (-10.0, 10.0)),
                                                     (3, 6, 3, 21, True, (-5.0, 5.0)), (1, 4, 2, 5, True, (0.0, 4.0)),
-                                                    (2, 300, 2, 200, False, (-1.0, 3.0)), (4, 33, 5, 2, True, (-2.0, 2.0))])
+                                                    (2, 300, 2, 200, False, (-1.0, 3.0)), (4, 33, 5, 2, True, (-2.0, 2.0)),
+                                                    (3, 9, 2, 1536, True, (-10.0, 10.0))])
 def test_dist_nstep_vs_oracle(T, B, N, n_atom, use_w, vr):
     need_cuda()
     g = rng(T + B + N + n_atom)
@@ -150,11 +152,12 @@ def run_qrdqn(inp, gamma, coef):
     return float(loss.item()), host(td), host(q.grad)
 
 
+# tau 1536: exactly 48 KB of dynamic shared memory, over the limit with the pairwise kernel's static shared memory
 @pytest.mark.parametrize("tau,T,B,N,use_w,use_vg", [(39, 10, 89, 67, False, True), (64, 5, 2000, 8, True, False),
                                                      (8, 5, 6, 4, False, False), (1, 1, 4, 1, True, False),
                                                      (32, 3, 100, 3, True, True), (33, 3, 50, 2, False, False),
                                                      (130, 2, 40, 2, True, False), (200, 1, 9, 1, False, True),
-                                                     (64, 2, 33, 20, False, False)])
+                                                     (64, 2, 33, 20, False, False), (1536, 1, 5, 2, True, False)])
 def test_qrdqn_vs_oracle(tau, T, B, N, use_w, use_vg):
     need_cuda()
     g = rng(tau * 3 + T + B + N)
@@ -203,13 +206,17 @@ def run_iqn(inp, gamma, kappa, coef):
     return float(loss.item()), host(td), host(q.grad)
 
 
+# (128, 28) and (127, 128): dynamic shared memory that fits the default limit only without the static shared memory
+# of the sorted (12.5 KB) and the pairwise kernel
 @pytest.mark.parametrize("tau,tau_p,T,B,N,kappa,use_w,use_vg", [(33, 34, 10, 64, 8, 0.9, False, True),
                                                                  (64, 64, 5, 2000, 8, 1.0, True, False),
                                                                  (8, 9, 5, 6, 4, 1.0, False, False),
                                                                  (1, 1, 1, 4, 1, 0.5, True, False),
                                                                  (32, 16, 3, 100, 3, 2.0, True, True),
                                                                  (70, 40, 2, 45, 2, 1.0, False, False),
-                                                                 (5, 130, 2, 33, 5, 1.0, True, False)])
+                                                                 (5, 130, 2, 33, 5, 1.0, True, False),
+                                                                 (128, 28, 3, 37, 2, 1.0, True, True),
+                                                                 (127, 128, 2, 33, 2, 1.0, False, False)])
 def test_iqn_vs_oracle(tau, tau_p, T, B, N, kappa, use_w, use_vg):
     need_cuda()
     g = rng(tau * 3 + tau_p + T + B + N)
@@ -242,11 +249,12 @@ def test_iqn_vs_golden(name):
         close_grad(gq, c.grad("q", prec), "grad_q")
 
 
-@pytest.mark.parametrize("n_atom", [2, 3, 4, 5, 31, 32, 33, 61, 62, 63, 64, 65, 127, 128, 129, 200])
+@pytest.mark.parametrize("n_atom", [2, 3, 4, 5, 31, 32, 33, 61, 62, 63, 64, 65, 114, 115, 116, 127, 128, 129, 200])
 def test_dist_atom_counts(n_atom):
     """every row length around the 32-atom segment / 4-float group boundaries of the TMA-gather kernel (rows start at
-    any of the four 16-byte phases: N * n_atom and the actions vary), a batch with a partial warp, and the hand-over to
-    the warp-per-sample kernel above 128 atoms"""
+    any of the four 16-byte phases: N * n_atom and the actions vary), a batch with a partial warp, the hand-over to
+    the warp-per-sample kernel above 128 atoms, and 114-116 atoms, whose dynamic shared memory fits 48 KB but not
+    together with the kernel's static shared memory"""
     need_cuda()
     g = rng(4000 + n_atom)
     T, B, N = 3, 77, 3
