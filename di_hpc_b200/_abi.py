@@ -38,6 +38,8 @@ SIGNATURES = {
     "hpc_rll_debug_host_schedule": (c_i64, [c_i64, c_i64, c_vp, c_i64]),
     "hpc_rll_gae_episodic_forward": (c_int, [c_vp] * 6 + [c_i64, c_i64, c_dbl, c_dbl, c_vp]),
     "hpc_rll_gae_episodic_backward": (c_int, [c_vp] * 6 + [c_i64, c_i64, c_dbl, c_dbl, c_vp]),
+    "hpc_rll_lambda_returns_forward": (c_int, [c_vp] * 6 + [c_i64] * 3 + [c_dbl, c_dbl, c_vp]),
+    "hpc_rll_lambda_returns_backward": (c_int, [c_vp] * 6 + [c_i64] * 3 + [c_dbl, c_dbl, c_vp]),
     "hpc_rll_device_numa_node": (c_int, [c_int]),
     "hpc_rll_bind_thread_to_device": (c_int, [c_int]),
     "hpc_rll_host_alloc": (c_vp, [c_sz, c_int]),
@@ -77,7 +79,7 @@ SIGNATURES = {
 SCATTER_COVER, SCATTER_ADD = 0, 1
 
 OP_GAE, OP_TD_LAMBDA, OP_VTRACE, OP_UPGO, OP_PPO, OP_Q_NSTEP_TD, OP_DIST_NSTEP_TD, OP_QRDQN_NSTEP_TD, \
-    OP_IQN_NSTEP_TD, OP_GAE_MOMENTS, OP_GAE_EPISODIC = range(11)
+    OP_IQN_NSTEP_TD, OP_GAE_MOMENTS, OP_GAE_EPISODIC, OP_LAMBDA_RETURNS = range(12)
 
 _lib = None
 

@@ -40,7 +40,7 @@ int sm_count() {
 static void init_cfg() {
     static const char* names[HPC_RLL_OP_COUNT] = {"GAE", "TD_LAMBDA", "VTRACE", "UPGO", "PPO",
                                                   "Q_NSTEP_TD", "DIST_NSTEP_TD", "QRDQN_NSTEP_TD", "IQN_NSTEP_TD",
-                                                  "GAE_MOMENTS", "GAE_EPISODIC"};
+                                                  "GAE_MOMENTS", "GAE_EPISODIC", "LAMBDA_RETURNS"};
     for (int i = 0; i < HPC_RLL_OP_COUNT; ++i) {
         char key[64];
         snprintf(key, sizeof(key), "HPC_RLL_CFG_%s", names[i]);
@@ -126,6 +126,10 @@ size_t hpc_rll_workspace_bytes(int op, int64_t T, int64_t B, int64_t N) {
 int hpc_rll_debug_set_config(int op, int cfg) {
     hpcrll::tuning_config(0);  // make sure env defaults were read first
     if (op < 0 || op >= HPC_RLL_OP_COUNT) return hpcrll::set_error(HPC_RLL_EINVAL, "bad op id %d", op);
+    // the λ-return op takes only the regimes it has (csrc/lambda_returns.cu), so a mistyped id cannot silently run
+    // another one
+    if (op == HPC_RLL_OP_LAMBDA_RETURNS && cfg != -1 && cfg != 21 && cfg != 33 && cfg != 99)
+        return hpcrll::set_error(HPC_RLL_EINVAL, "op %d: unknown config %d (-1, 21, 33 or 99)", op, cfg);
     hpcrll::g_cfg[op].store(cfg);
     return HPC_RLL_OK;
 }

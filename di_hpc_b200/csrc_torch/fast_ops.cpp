@@ -105,6 +105,56 @@ struct GaeEpisodicFn : public Function<GaeEpisodicFn> {
     }
 };
 
+// ------------------------------------------------------------------------------------------------ λ-returns
+// gammas / lambdas: a (T,B) fp32 tensor, or undefined for the scalar gamma / lambda.  offset: the first row of
+// bootstrap_values a return reads (1 for generalized_lambda_returns, 0 for multistep_forward_view).
+inline Tensor opt_tb(const OptTensor& t, const char* name, const Tensor& like) {
+    const Tensor x = opt_f32(t, name);
+    TORCH_CHECK_VALUE(!x.defined() || (x.sizes() == like.sizes() && x.device() == like.device()), name,
+                      " must be a number or a (T, B)=", like.sizes(), " tensor on the device of rewards");
+    return x;
+}
+
+struct LambdaReturnsFn : public Function<LambdaReturnsFn> {
+    static Tensor forward(AutogradContext* ctx, const Tensor& bootstrap_, const Tensor& rewards_,
+                          const OptTensor& gammas_, const OptTensor& lambdas_, const OptTensor& done_, double gamma,
+                          double lambda, int64_t offset) {
+        const Tensor rewards = f32(rewards_, "rewards"), bootstrap = f32(bootstrap_, "bootstrap_values");
+        TORCH_CHECK_VALUE(rewards.dim() == 2, "rewards must be (T, B), got ", rewards.sizes());
+        const int64_t T = rewards.size(0), B = rewards.size(1);
+        TORCH_CHECK_VALUE(bootstrap.dim() == 2 && bootstrap.size(0) == T + offset && bootstrap.size(1) == B,
+                          "bootstrap_values must be (", T + offset, ", ", B, "), got ", bootstrap.sizes());
+        TORCH_CHECK_VALUE(bootstrap.device() == rewards.device(), "bootstrap_values and rewards must be on one device");
+        const Tensor gammas = opt_tb(gammas_, "gammas", rewards), lambdas = opt_tb(lambdas_, "lambda_", rewards);
+        const Tensor done = mask_u8(done_, "done", rewards);
+        c10::cuda::CUDAGuard guard(rewards.device());
+        Tensor ret = torch::empty_like(rewards);
+        ck(hpc_rll_lambda_returns_forward(fp(bootstrap), fp(rewards), fp(gammas), fp(lambdas), u8p(done), fpm(ret), T,
+                                          B, offset, gamma, lambda, cur_stream()),
+           "hpc_rll_lambda_returns_forward");
+        ctx->save_for_backward({gammas, lambdas, done});
+        ctx->saved_data["gamma"] = gamma;
+        ctx->saved_data["lambda"] = lambda;
+        ctx->saved_data["offset"] = offset;
+        return ret;
+    }
+    static variable_list backward(AutogradContext* ctx, variable_list grads) {
+        const auto sv = ctx->get_saved_variables();
+        const Tensor &gammas = sv[0], &lambdas = sv[1], &done = sv[2];
+        const Tensor g = f32(grads[0], "grad_returns");
+        const int64_t T = g.size(0), B = g.size(1), offset = ctx->saved_data["offset"].toInt();
+        c10::cuda::CUDAGuard guard(g.device());
+        // one pass writes both gradients; the ABI zeroes the leading bootstrap row, which with T == 0 it does not reach
+        Tensor gb = T == 0 ? torch::zeros({offset, B}, g.options()) : torch::empty({T + offset, B}, g.options());
+        Tensor gr = torch::empty_like(g);
+        ck(hpc_rll_lambda_returns_backward(fp(g), fp(gammas), fp(lambdas), u8p(done), fpm(gb), fpm(gr), T, B, offset,
+                                           ctx->saved_data["gamma"].toDouble(), ctx->saved_data["lambda"].toDouble(),
+                                           cur_stream()),
+           "hpc_rll_lambda_returns_backward");
+        return {gb, gr, Tensor(), Tensor(), Tensor(), Tensor(), Tensor(), Tensor()};
+    }
+};
+
 // ------------------------------------------------------------------------------------------------ TD(lambda)
 struct TdLambdaFn : public Function<TdLambdaFn> {
     static Tensor forward(AutogradContext* ctx, const Tensor& value_, const Tensor& reward_, const OptTensor& weight_,
@@ -541,6 +591,13 @@ void register_fast_ops(pybind11::module& m) {
           [](const Tensor& v, const Tensor& nv, const Tensor& r, const OptTensor& done, const OptTensor& traj, double g,
              double l) { return GaeEpisodicFn::apply(v, nv, r, done, traj, g, l); },
           "episode-aware (un-normalised) GAE with done / traj_flag masks, with autograd (adjoint)");
+    m.def("lambda_returns",
+          [](const Tensor& v, const Tensor& r, const OptTensor& gammas, const OptTensor& lambdas,
+             const OptTensor& done, double g, double l, int64_t offset) {
+              return LambdaReturnsFn::apply(v, r, gammas, lambdas, done, g, l, offset);
+          },
+          "lambda-returns with per-step (or scalar) gamma / lambda and a done mask, with autograd (adjoint); "
+          "bootstrap_values rows from `offset` on are the V_t");
     m.def("td_lambda",
           [](const Tensor& v, const Tensor& r, const OptTensor& w, double g, double l, int64_t gb) {
               return TdLambdaFn::apply(v, r, w, g, l, gb);

@@ -1,4 +1,5 @@
 from di_hpc_b200.rl_utils.td import (DistNStepTD, DistNStepTDFunction, IQNNStepTDError,  # noqa: F401
                                       IQNNStepTDErrorFunction, QNStepTD, QNStepTDFunction, QNStepTDRescale,
                                       QNStepTDRescaleFunction, QRDQNNStepTDError, QRDQNNStepTDErrorFunction,
-                                      TDLambda, TDLambdaFunction)
+                                      TDLambda, TDLambdaFunction, generalized_lambda_returns,
+                                      multistep_forward_view)

@@ -48,7 +48,8 @@ extern "C" {
 #define HPC_RLL_OP_IQN_NSTEP_TD 8
 #define HPC_RLL_OP_GAE_MOMENTS 9 /* workspace sizing only; tuning follows HPC_RLL_OP_GAE */
 #define HPC_RLL_OP_GAE_EPISODIC 10
-#define HPC_RLL_OP_COUNT 11
+#define HPC_RLL_OP_LAMBDA_RETURNS 11
+#define HPC_RLL_OP_COUNT 12
 
 /* ---- library ------------------------------------------------------------------------------ */
 const char* hpc_rll_version(void);
@@ -57,7 +58,8 @@ const char* hpc_rll_last_error(void); /* thread-local, valid until the next fail
 uint64_t hpc_rll_launch_count(void);
 /* scratch bytes an op needs for sizes (T,B,N); N = action dim / n_atom / tau as relevant */
 size_t hpc_rll_workspace_bytes(int op, int64_t T, int64_t B, int64_t N);
-/* tuning/debug: force kernel configuration `cfg` for `op` (-1 = automatic) */
+/* tuning/debug: force kernel configuration `cfg` for `op` (-1 = automatic); HPC_RLL_OP_LAMBDA_RETURNS accepts only
+ * -1, 21 (look-back), 33 (wide) and 99 (generic) */
 int hpc_rll_debug_set_config(int op, int cfg);
 
 /* out[i] = a[0]*x[i] + b[0]*y[i]  (a, b DEVICE scalars; b and y may be NULL together: out = a[0]*x).  Glue for
@@ -141,6 +143,30 @@ int hpc_rll_gae_episodic_forward(const float* value, const float* next_value, co
 int hpc_rll_gae_episodic_backward(const float* grad_adv, const uint8_t* done_u8, const uint8_t* traj_u8,
                                   float* grad_value, float* grad_next_value, float* grad_reward, int64_t T, int64_t B,
                                   double gamma, double lambda, void* stream);
+
+/* ---- λ-returns ------------------------------------------------------------------------------------
+ * DI-engine's generalized_lambda_returns / multistep_forward_view with per-step discounts and episode ends.  The
+ * reference computes them in Python only (hpc_rll/origin/td.py); the library's TD(lambda) loss has no returns output.
+ *   bootstrap_values (T+bootstrap_offset, B): V_t = bootstrap_values[t + bootstrap_offset], offset 1 for
+ *     generalized_lambda_returns ((T+1,B) values), 0 for multistep_forward_view ((T,B) values of the next states)
+ *   rewards (T,B) fp32; gammas, lambdas (T,B) fp32 or NULL (= the scalar `gamma` / `lambda`, rounded to fp32);
+ *   done_u8 (T,B) bytes, non-zero = set, or NULL (absent).  With d = gamma*lambda, e = gamma - d (fp32) and
+ *   m = 0 where done is set, 1 elsewhere:
+ *     done absent:  R_{T-1} = r + gamma*V,        R_t = (r_t + d_t*R_{t+1}) + e_t*V_t
+ *     done given:   R_{T-1} = r + (m*gamma)*V,    R_t = r_t + m_t*(d_t*R_{t+1} + e_t*V_t)
+ * backward: grad_returns (T,B) -> grad_bootstrap_values (T+bootstrap_offset, B), grad_rewards (T,B), all written
+ * (the rows before bootstrap_offset are zeroed):
+ *     u_0 = G_0,  u_t = G_t + u_{t-1}*d_{t-1}  (done given: (u_{t-1}*m_{t-1})*d_{t-1})
+ *     grad_rewards = u,  grad_V_t = u_t*e_t  (done given: (u_t*m_t)*e_t);  row T-1: u*gamma  (done given: u*(m*gamma))
+ * Every product is one rounded fp32 operation in this order.  All tensors contiguous.  A data pointer may be NULL only
+ * when T*B == 0. */
+int hpc_rll_lambda_returns_forward(const float* bootstrap_values, const float* rewards, const float* gammas,
+                                   const float* lambdas, const uint8_t* done_u8, float* returns, int64_t T, int64_t B,
+                                   int64_t bootstrap_offset, double gamma, double lambda, void* stream);
+int hpc_rll_lambda_returns_backward(const float* grad_returns, const float* gammas, const float* lambdas,
+                                    const uint8_t* done_u8, float* grad_bootstrap_values, float* grad_rewards,
+                                    int64_t T, int64_t B, int64_t bootstrap_offset, double gamma, double lambda,
+                                    void* stream);
 
 /* test hook: the stage heights hpc_rll_gae_fwd_bwd_host would use for a (T,B) problem (host-only, no CUDA call);
  * writes up to `cap` entries, returns the number of stages */
