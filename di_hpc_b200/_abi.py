@@ -40,6 +40,10 @@ SIGNATURES = {
     "hpc_rll_gae_episodic_backward": (c_int, [c_vp] * 6 + [c_i64, c_i64, c_dbl, c_dbl, c_vp]),
     "hpc_rll_lambda_returns_forward": (c_int, [c_vp] * 6 + [c_i64] * 3 + [c_dbl, c_dbl, c_vp]),
     "hpc_rll_lambda_returns_backward": (c_int, [c_vp] * 6 + [c_i64] * 3 + [c_dbl, c_dbl, c_vp]),
+    "hpc_rll_vtrace_return_forward": (c_int, [c_vp] * 5 + [c_i64, c_i64, c_dbl, c_dbl, c_vp]),
+    "hpc_rll_vtrace_return_backward": (c_int, [c_vp] * 5 + [c_i64, c_i64, c_dbl, c_dbl, c_vp]),
+    "hpc_rll_upgo_returns_forward": (c_int, [c_vp] * 4 + [c_i64, c_i64, c_vp]),
+    "hpc_rll_upgo_returns_backward": (c_int, [c_vp] * 4 + [c_i64, c_i64, c_vp]),
     "hpc_rll_device_numa_node": (c_int, [c_int]),
     "hpc_rll_bind_thread_to_device": (c_int, [c_int]),
     "hpc_rll_host_alloc": (c_vp, [c_sz, c_int]),

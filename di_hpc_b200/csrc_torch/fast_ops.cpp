@@ -155,6 +155,89 @@ struct LambdaReturnsFn : public Function<LambdaReturnsFn> {
     }
 };
 
+// ------------------------------------------------------------------------------------------------ V-trace / UPGO returns
+// (T+1, B) bootstrap values of (T, B) rewards, on their device
+inline Tensor bootstrap_of(const Tensor& b_, const Tensor& rewards, const char* rname) {
+    const Tensor b = f32(b_, "bootstrap_values");
+    const int64_t T = rewards.size(0), B = rewards.size(1);
+    TORCH_CHECK_VALUE(b.dim() == 2 && b.size(0) == T + 1 && b.size(1) == B, "bootstrap_values must be (", T + 1, ", ",
+                      B, "), got ", b.sizes());
+    TORCH_CHECK_VALUE(b.device() == rewards.device(), "bootstrap_values and ", rname, " must be on one device");
+    return b;
+}
+
+// gradients flow to reward and bootstrap_values; clipped_rhos / clipped_cs are constants (checked in Python)
+struct VtraceReturnFn : public Function<VtraceReturnFn> {
+    static Tensor forward(AutogradContext* ctx, const Tensor& rhos_, const Tensor& cs_, const Tensor& reward_,
+                          const Tensor& bootstrap_, double gamma, double lambda) {
+        const Tensor reward = f32(reward_, "reward");
+        TORCH_CHECK_VALUE(reward.dim() == 2, "reward must be (T, B), got ", reward.sizes());
+        const Tensor bootstrap = bootstrap_of(bootstrap_, reward, "reward");
+        const auto like_reward = [&](const Tensor& x_, const char* name) {
+            const Tensor x = f32(x_, name);
+            TORCH_CHECK_VALUE(x.sizes() == reward.sizes() && x.device() == reward.device(), name, " must be a (T, B)=",
+                              reward.sizes(), " tensor on the device of reward, got ", x.sizes());
+            return x;
+        };
+        const Tensor rhos = like_reward(rhos_, "clipped_rhos"), cs = like_reward(cs_, "clipped_cs");
+        const int64_t T = reward.size(0), B = reward.size(1);
+        c10::cuda::CUDAGuard guard(reward.device());
+        Tensor ret = torch::empty_like(reward);
+        ck(hpc_rll_vtrace_return_forward(fp(rhos), fp(cs), fp(reward), fp(bootstrap), fpm(ret), T, B, gamma, lambda,
+                                         cur_stream()),
+           "hpc_rll_vtrace_return_forward");
+        ctx->save_for_backward({rhos, cs});
+        ctx->saved_data["gamma"] = gamma;
+        ctx->saved_data["lambda"] = lambda;
+        return ret;
+    }
+    static variable_list backward(AutogradContext* ctx, variable_list grads) {
+        const auto sv = ctx->get_saved_variables();
+        const Tensor &rhos = sv[0], &cs = sv[1];
+        const Tensor g = f32(grads[0], "grad_returns");
+        const int64_t T = g.size(0), B = g.size(1);
+        c10::cuda::CUDAGuard guard(g.device());
+        // one pass writes both gradients, row T of bootstrap_values included; with T == 0 nothing runs
+        Tensor gb = T == 0 ? torch::zeros({1, B}, g.options()) : torch::empty({T + 1, B}, g.options());
+        Tensor gr = torch::empty_like(g);
+        ck(hpc_rll_vtrace_return_backward(fp(g), fp(rhos), fp(cs), fpm(gr), fpm(gb), T, B,
+                                          ctx->saved_data["gamma"].toDouble(), ctx->saved_data["lambda"].toDouble(),
+                                          cur_stream()),
+           "hpc_rll_vtrace_return_backward");
+        return {Tensor(), Tensor(), gr, gb, Tensor(), Tensor()};
+    }
+};
+
+// save_mask: keep the (T,B) ℓ bytes for the backward (only when a gradient will be asked for)
+struct UpgoReturnsFn : public Function<UpgoReturnsFn> {
+    static Tensor forward(AutogradContext* ctx, const Tensor& rewards_, const Tensor& bootstrap_, bool save_mask) {
+        const Tensor rewards = f32(rewards_, "rewards");
+        TORCH_CHECK_VALUE(rewards.dim() == 2, "rewards must be (T, B), got ", rewards.sizes());
+        const Tensor bootstrap = bootstrap_of(bootstrap_, rewards, "rewards");
+        const int64_t T = rewards.size(0), B = rewards.size(1);
+        c10::cuda::CUDAGuard guard(rewards.device());
+        Tensor ret = torch::empty_like(rewards);
+        Tensor mask = save_mask ? torch::empty({T, B}, rewards.options().dtype(torch::kUInt8)) : Tensor();
+        ck(hpc_rll_upgo_returns_forward(fp(rewards), fp(bootstrap), fpm(ret),
+                                        mask.defined() ? mask.data_ptr<uint8_t>() : nullptr, T, B, cur_stream()),
+           "hpc_rll_upgo_returns_forward");
+        ctx->save_for_backward({mask});
+        return ret;
+    }
+    static variable_list backward(AutogradContext* ctx, variable_list grads) {
+        const Tensor mask = ctx->get_saved_variables()[0];
+        TORCH_CHECK(mask.defined(), "upgo_returns: backward through a call made without gradients");
+        const Tensor g = f32(grads[0], "grad_returns");
+        const int64_t T = g.size(0), B = g.size(1);
+        c10::cuda::CUDAGuard guard(g.device());
+        Tensor gb = T == 0 ? torch::zeros({1, B}, g.options()) : torch::empty({T + 1, B}, g.options());
+        Tensor gr = torch::empty_like(g);
+        ck(hpc_rll_upgo_returns_backward(fp(g), u8p(mask), fpm(gr), fpm(gb), T, B, cur_stream()),
+           "hpc_rll_upgo_returns_backward");
+        return {gr, gb, Tensor()};
+    }
+};
+
 // ------------------------------------------------------------------------------------------------ TD(lambda)
 struct TdLambdaFn : public Function<TdLambdaFn> {
     static Tensor forward(AutogradContext* ctx, const Tensor& value_, const Tensor& reward_, const OptTensor& weight_,
@@ -598,6 +681,15 @@ void register_fast_ops(pybind11::module& m) {
           },
           "lambda-returns with per-step (or scalar) gamma / lambda and a done mask, with autograd (adjoint); "
           "bootstrap_values rows from `offset` on are the V_t");
+    m.def("vtrace_nstep_return",
+          [](const Tensor& rhos, const Tensor& cs, const Tensor& r, const Tensor& v, double g, double l) {
+              return VtraceReturnFn::apply(rhos, cs, r, v, g, l);
+          },
+          "V-trace target v_s with autograd (adjoint) in reward and bootstrap_values");
+    m.def("upgo_returns",
+          [](const Tensor& r, const Tensor& v, bool save_mask) { return UpgoReturnsFn::apply(r, v, save_mask); },
+          "UPGO returns with autograd (adjoint) in rewards and bootstrap_values; save_mask keeps the lambda mask "
+          "the backward reads");
     m.def("td_lambda",
           [](const Tensor& v, const Tensor& r, const OptTensor& w, double g, double l, int64_t gb) {
               return TdLambdaFn::apply(v, r, w, g, l, gb);

@@ -48,3 +48,29 @@ class UPGO(torch.nn.Module):
         assert (rewards.is_cuda)
         assert (bootstrap_values.is_cuda)
         return UpgoFunction.apply(target_output, rhos, action, rewards, bootstrap_values, self.global_B)
+
+
+def upgo_returns(rewards, bootstrap_values):
+    r"""
+    Overview:
+        UPGO return targets of a ``(T, B)`` rollout segment, as DI-engine's ``upgo_returns``
+        (hpc_rll/origin/upgo.py:21-38): a λ-return with γ = 1 whose trace continues (``ℓ_t = 1``) while the next step
+        did at least as well as its value estimate.  With ``V_t = bootstrap_values[t]``::
+
+            ℓ_t = [r_{t+1} + V_{t+2} >= V_{t+1}]   (t < T−1; a NaN compares false)
+            R_{T−1} = r_{T−1} + V_T                R_t = (r_t + ℓ_t·R_{t+1}) + (1 − ℓ_t)·V_{t+1}
+
+        Every operation is one rounded fp32 operation in this order, so the result and its gradients match origin bit
+        for bit; long, narrow batches (B <= 2048, T >= 512) are scanned in parallel pieces and agree to ~1e-7 relative
+        instead.  Differentiable in ``rewards`` and ``bootstrap_values`` (ℓ is not differentiated, and the gradient of
+        ``bootstrap_values[0]`` is +0).  When a gradient may be asked for, the call keeps ℓ as one byte per element
+        for the backward.
+    Arguments:
+        - rewards (:obj:`torch.FloatTensor`): :math:`(T, B)`
+        - bootstrap_values (:obj:`torch.FloatTensor`): :math:`(T + 1, B)`, the value estimates of steps 0 to T
+    Returns:
+        - return (:obj:`torch.FloatTensor`): :math:`(T, B)`
+    """
+    save_mask = torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad
+                                                for x in (rewards, bootstrap_values))
+    return _ext.require().upgo_returns(rewards, bootstrap_values, save_mask)

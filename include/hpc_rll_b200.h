@@ -168,6 +168,33 @@ int hpc_rll_lambda_returns_backward(const float* grad_returns, const float* gamm
                                     int64_t T, int64_t B, int64_t bootstrap_offset, double gamma, double lambda,
                                     void* stream);
 
+/* ---- V-trace and UPGO returns ------------------------------------------------------------------
+ * The recursions inside the V-trace and UPGO losses as standalone ops (hpc_rll/origin/vtrace.py:5-13 vtrace_nstep_return,
+ * hpc_rll/origin/upgo.py:21-38 upgo_returns).  reward / rewards (T,B), bootstrap_values (T+1,B), V_t =
+ * bootstrap_values[t]; returns (T,B).  Members of the λ-return family: HPC_RLL_OP_LAMBDA_RETURNS selects their kernels.
+ * V-trace, with g = fp32(gamma), f = fp32(gamma*lambda) (the product in double) and rhos, cs (T,B) the clipped ratios:
+ *     a_t = (r_t + g*V_{t+1}) - V_t,  item_T = +0,  item_t = rho_t*a_t + (f*c_t)*item_{t+1},  R_t = V_t + item_t
+ *   backward: grad_returns -> grad_reward (T,B), grad_bootstrap_values (T+1,B), all written:
+ *     w_0 = G_0,  w_t = G_t + (f*c_{t-1})*w_{t-1},  p_t = w_t*rho_t,  grad_reward = p
+ *     grad_V_t = (G_t - p_t) + g*p_{t-1}  (grad_V_0 = G_0 - p_0),  grad_V_T = g*p_{T-1}
+ * UPGO, with l_t = [r_{t+1} + V_{t+2} >= V_{t+1}] for t < T-1 (0 when the comparison has a NaN), l_{T-1} = 0:
+ *     R_{T-1} = r_{T-1} + V_T,  R_t = (r_t + l_t*R_{t+1}) + (1 - l_t)*V_{t+1}
+ *   lambda_mask (T,B) bytes: the forward writes l there (1 or 0) unless it is NULL; the backward reads it (non-zero =
+ *   set) and writes grad_rewards (T,B) and grad_bootstrap_values (T+1,B), row 0 zeroed:
+ *     u_0 = G_0,  u_t = G_t + l_{t-1}*u_{t-1},  grad_rewards = u,  grad_V_{t+1} = u_t*(1 - l_t)
+ * Every product is one rounded fp32 operation in this order.  All tensors contiguous.  A data pointer may be NULL only
+ * when T*B == 0. */
+int hpc_rll_vtrace_return_forward(const float* rhos, const float* cs, const float* reward,
+                                  const float* bootstrap_values, float* returns, int64_t T, int64_t B, double gamma,
+                                  double lambda, void* stream);
+int hpc_rll_vtrace_return_backward(const float* grad_returns, const float* rhos, const float* cs, float* grad_reward,
+                                   float* grad_bootstrap_values, int64_t T, int64_t B, double gamma, double lambda,
+                                   void* stream);
+int hpc_rll_upgo_returns_forward(const float* rewards, const float* bootstrap_values, float* returns,
+                                 uint8_t* lambda_mask, int64_t T, int64_t B, void* stream);
+int hpc_rll_upgo_returns_backward(const float* grad_returns, const uint8_t* lambda_mask, float* grad_rewards,
+                                  float* grad_bootstrap_values, int64_t T, int64_t B, void* stream);
+
 /* test hook: the stage heights hpc_rll_gae_fwd_bwd_host would use for a (T,B) problem (host-only, no CUDA call);
  * writes up to `cap` entries, returns the number of stages */
 int64_t hpc_rll_debug_host_schedule(int64_t T, int64_t B, int64_t* rows, int64_t cap);
