@@ -44,6 +44,10 @@ SIGNATURES = {
     "hpc_rll_vtrace_return_backward": (c_int, [c_vp] * 5 + [c_i64, c_i64, c_dbl, c_dbl, c_vp]),
     "hpc_rll_upgo_returns_forward": (c_int, [c_vp] * 4 + [c_i64, c_i64, c_vp]),
     "hpc_rll_upgo_returns_backward": (c_int, [c_vp] * 4 + [c_i64, c_i64, c_vp]),
+    "hpc_rll_importance_weights_forward": (c_int, [c_vp] * 4 + [c_i64, c_i64, c_vp]),
+    "hpc_rll_importance_weights_backward": (c_int, [c_vp] * 7 + [c_i64, c_i64, c_vp, c_sz, c_vp]),
+    "hpc_rll_tb_cross_entropy_forward": (c_int, [c_vp] * 3 + [c_i64, c_i64, c_vp]),
+    "hpc_rll_tb_cross_entropy_backward": (c_int, [c_vp] * 4 + [c_i64, c_i64, c_vp]),
     "hpc_rll_device_numa_node": (c_int, [c_int]),
     "hpc_rll_bind_thread_to_device": (c_int, [c_int]),
     "hpc_rll_host_alloc": (c_vp, [c_sz, c_int]),
@@ -83,7 +87,7 @@ SIGNATURES = {
 SCATTER_COVER, SCATTER_ADD = 0, 1
 
 OP_GAE, OP_TD_LAMBDA, OP_VTRACE, OP_UPGO, OP_PPO, OP_Q_NSTEP_TD, OP_DIST_NSTEP_TD, OP_QRDQN_NSTEP_TD, \
-    OP_IQN_NSTEP_TD, OP_GAE_MOMENTS, OP_GAE_EPISODIC, OP_LAMBDA_RETURNS = range(12)
+    OP_IQN_NSTEP_TD, OP_GAE_MOMENTS, OP_GAE_EPISODIC, OP_LAMBDA_RETURNS, OP_IMPORTANCE_WEIGHTS = range(13)
 
 _lib = None
 

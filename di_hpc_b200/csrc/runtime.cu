@@ -40,7 +40,8 @@ int sm_count() {
 static void init_cfg() {
     static const char* names[HPC_RLL_OP_COUNT] = {"GAE", "TD_LAMBDA", "VTRACE", "UPGO", "PPO",
                                                   "Q_NSTEP_TD", "DIST_NSTEP_TD", "QRDQN_NSTEP_TD", "IQN_NSTEP_TD",
-                                                  "GAE_MOMENTS", "GAE_EPISODIC", "LAMBDA_RETURNS"};
+                                                  "GAE_MOMENTS", "GAE_EPISODIC", "LAMBDA_RETURNS",
+                                                  "IMPORTANCE_WEIGHTS"};
     for (int i = 0; i < HPC_RLL_OP_COUNT; ++i) {
         char key[64];
         snprintf(key, sizeof(key), "HPC_RLL_CFG_%s", names[i]);
@@ -130,6 +131,9 @@ int hpc_rll_debug_set_config(int op, int cfg) {
     // another one
     if (op == HPC_RLL_OP_LAMBDA_RETURNS && cfg != -1 && cfg != 21 && cfg != 33 && cfg != 99)
         return hpcrll::set_error(HPC_RLL_EINVAL, "op %d: unknown config %d (-1, 21, 33 or 99)", op, cfg);
+    // the importance-weights id sizes a workspace only: its row kernels follow the row length, there is nothing to tune
+    if (op == HPC_RLL_OP_IMPORTANCE_WEIGHTS)
+        return hpcrll::set_error(HPC_RLL_EINVAL, "op %d: unknown config %d (the op has no tuning configs)", op, cfg);
     hpcrll::g_cfg[op].store(cfg);
     return HPC_RLL_OK;
 }

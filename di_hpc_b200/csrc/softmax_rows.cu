@@ -4,6 +4,8 @@
 // Replaces vtraceBackwardTargetOutput (include/hpc/rll/cuda/rl_utils/vtrace_kernel.h:235-273),
 // upgoBackwardKernel (upgo_kernel.h:96-108) and ppoBackwardLogitsNew (ppo_kernel.h:252-283), which
 // re-read (T,B,N) buffers saved by the forward; here the softmax is recomputed from the logits.
+#include <atomic>
+
 #include "softmax_rows.cuh"
 
 namespace hpcrll {
@@ -183,6 +185,21 @@ int launch_softmax_grad_rows(const float* logits, const int64_t* action, const f
     // bit-identical.
     return launch_rows<GradRows>(&grid, R, N, logits, grad, stream, logits, action, c1, static_cast<const float*>(nullptr),
                                  g1, g1, 0.f, grad);
+}
+
+__device__ float g_unit_scalars[2] = {1.f, -1.f};
+
+int unit_scalars(const float** out) {
+    constexpr int kMaxDevices = 64;
+    static std::atomic<const float*> cache[kMaxDevices] = {};
+    int dev = 0;
+    HPC_CUDA(cudaGetDevice(&dev));
+    if (dev < kMaxDevices && (*out = cache[dev].load(std::memory_order_acquire)) != nullptr) return HPC_RLL_OK;
+    void* p = nullptr;
+    HPC_CUDA(cudaGetSymbolAddress(&p, g_unit_scalars));
+    *out = static_cast<const float*>(p);
+    if (dev < kMaxDevices) cache[dev].store(*out, std::memory_order_release);
+    return HPC_RLL_OK;
 }
 
 // ---- fixed-order finaliser for several loss terms with different partial counts ---------------------

@@ -424,6 +424,11 @@ int launch_softmax_grad_rows(const float* logits, const int64_t* action, const f
                              const float* g1, const float* g2, double inv_n, float* grad, int64_t R, int64_t N,
                              cudaStream_t stream);
 
+// *out = the library's device constants {+1, -1} on the current device: the fixed upstream scale g1 of a
+// launch_softmax_grad_rows call.  The address is looked up once per device and cached, so a call made once eagerly
+// leaves nothing to resolve while a stream is being captured.
+int unit_scalars(const float** out);
+
 // grid size for a row-streaming kernel: enough CTAs to fill the machine, grid-stride over row blocks
 inline unsigned rows_grid(int64_t R, int rows_per_block) {
     int64_t blocks = (R + rows_per_block - 1) / rows_per_block;

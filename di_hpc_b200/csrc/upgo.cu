@@ -298,4 +298,34 @@ int hpc_rll_upgo_backward(const float* grad_loss, const float* target_output, co
                                     grad_target_output, T * B, N, as_stream(stream_));
 }
 
+// tb_cross_entropy (hpc_rll/origin/upgo.py:7-18): UPGO's `metric` as a standalone op, through the same row kernels
+int hpc_rll_tb_cross_entropy_forward(const float* logit, const int64_t* label, float* out, int64_t R, int64_t N,
+                                     void* stream_) {
+    HPC_NVTX("tb_cross_entropy_forward");
+    using namespace hpcrll;
+    HPC_REQUIRE(R >= 0, "tb_cross_entropy_forward: negative row count R=%lld", (long long)R);
+    HPC_REQUIRE(N > 0 && N < (int64_t(1) << 30), "tb_cross_entropy_forward: the row length N must be in [1, 2^30), "
+                "got %lld", (long long)N);
+    if (R == 0) return HPC_RLL_OK;
+    HPC_REQUIRE(logit && label && out, "tb_cross_entropy_forward: null logit, label or out pointer");
+    unsigned grid;
+    return launch_rows<UpgoRows>(&grid, R, N, logit, nullptr, as_stream(stream_), logit, label, out);
+}
+
+int hpc_rll_tb_cross_entropy_backward(const float* grad_out, const float* logit, const int64_t* label,
+                                      float* grad_logit, int64_t R, int64_t N, void* stream_) {
+    HPC_NVTX("tb_cross_entropy_backward");
+    using namespace hpcrll;
+    HPC_REQUIRE(R >= 0, "tb_cross_entropy_backward: negative row count R=%lld", (long long)R);
+    HPC_REQUIRE(N > 0 && N < (int64_t(1) << 30), "tb_cross_entropy_backward: the row length N must be in [1, 2^30), "
+                "got %lld", (long long)N);
+    if (R == 0) return HPC_RLL_OK;
+    HPC_REQUIRE(grad_out && logit && label && grad_logit,
+                "tb_cross_entropy_backward: null grad_out, logit, label or grad_logit pointer");
+    const float* one;  // {+1, -1}: the upstream gradient is the per-row c1, scaled by +1
+    if (int rc = unit_scalars(&one)) return rc;
+    return launch_softmax_grad_rows(logit, label, grad_out, nullptr, one, nullptr, 0.0, grad_logit, R, N,
+                                    as_stream(stream_));
+}
+
 }  // extern "C"

@@ -10,6 +10,7 @@ size_t vtrace_workspace_bytes(int64_t T, int64_t B);
 size_t upgo_workspace_bytes(int64_t T, int64_t B);
 size_t ppo_workspace_bytes();
 size_t nstep_workspace_bytes();
+size_t importance_weights_workspace_bytes(int64_t R);
 
 size_t workspace_bytes(int op, int64_t T, int64_t B, int64_t N) {
     (void)T;
@@ -33,6 +34,8 @@ size_t workspace_bytes(int op, int64_t T, int64_t B, int64_t N) {
         case HPC_RLL_OP_QRDQN_NSTEP_TD:
         case HPC_RLL_OP_IQN_NSTEP_TD:
             return nstep_workspace_bytes();
+        case HPC_RLL_OP_IMPORTANCE_WEIGHTS:
+            return importance_weights_workspace_bytes(T * B);
         default:
             return 0;
     }

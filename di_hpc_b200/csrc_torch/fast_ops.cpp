@@ -238,6 +238,82 @@ struct UpgoReturnsFn : public Function<UpgoReturnsFn> {
     }
 };
 
+// ------------------------------------------------------------------------------------------------ importance weights
+// target / behaviour (*, N) logits, action (*) int64 -> rho (*).  save: keep what the backward reads (only when a
+// gradient may be asked for)
+struct ImportanceWeightsFn : public Function<ImportanceWeightsFn> {
+    static Tensor forward(AutogradContext* ctx, const Tensor& target_, const Tensor& behaviour_, const Tensor& action_,
+                          bool save) {
+        const Tensor target = f32(target_, "target_output"), behaviour = f32(behaviour_, "behaviour_output");
+        const Tensor action = i64(action_, "action");
+        TORCH_CHECK_VALUE(target.dim() >= 1 && target.size(-1) >= 1, "target_output must be (*, N) with N >= 1, got ",
+                          target.sizes());
+        TORCH_CHECK_VALUE(behaviour.sizes() == target.sizes(), "behaviour_output must have the shape of target_output ",
+                          target.sizes(), ", got ", behaviour.sizes());
+        TORCH_CHECK_VALUE(action.sizes() == target.sizes().slice(0, target.dim() - 1), "action must be ",
+                          target.sizes().slice(0, target.dim() - 1), ", got ", action.sizes());
+        TORCH_CHECK_VALUE(behaviour.device() == target.device() && action.device() == target.device(),
+                          "target_output, behaviour_output and action must be on one device");
+        const int64_t R = action.numel(), N = target.size(-1);
+        c10::cuda::CUDAGuard guard(target.device());
+        Tensor rho = torch::empty(action.sizes(), target.options());
+        ck(hpc_rll_importance_weights_forward(fp(target), fp(behaviour), ip(action), fpm(rho), R, N, cur_stream()),
+           "hpc_rll_importance_weights_forward");
+        if (save) ctx->save_for_backward({target, behaviour, action, rho});
+        return rho;
+    }
+    static variable_list backward(AutogradContext* ctx, variable_list grads) {
+        const auto sv = ctx->get_saved_variables();
+        TORCH_CHECK(!sv.empty(), "compute_importance_weights: backward through a call made without gradients");
+        const Tensor &target = sv[0], &behaviour = sv[1], &action = sv[2], &rho = sv[3];
+        const bool want_t = ctx->needs_input_grad(0), want_b = ctx->needs_input_grad(1);
+        if (!grads[0].defined() || !(want_t || want_b)) return {Tensor(), Tensor(), Tensor(), Tensor()};
+        const Tensor g = f32(grads[0], "grad_rho");
+        const int64_t R = action.numel(), N = target.size(-1);
+        c10::cuda::CUDAGuard guard(target.device());
+        Tensor gt = want_t ? torch::empty_like(target) : Tensor();
+        Tensor gb = want_b ? torch::empty_like(behaviour) : Tensor();
+        Tensor ws = workspace(HPC_RLL_OP_IMPORTANCE_WEIGHTS, R, 1, N, target);
+        ck(hpc_rll_importance_weights_backward(fp(g), fp(target), fp(behaviour), ip(action), fp(rho), fpm(gt), fpm(gb),
+                                               R, N, ws.data_ptr(), ws.numel(), cur_stream()),
+           "hpc_rll_importance_weights_backward");
+        return {gt, gb, Tensor(), Tensor()};
+    }
+};
+
+// ------------------------------------------------------------------------------------------------ tb_cross_entropy
+// logit: T*B rows of N (any shape with last dim N, as origin's reshape(-1, N)); label (T,B) int64 -> (T,B)
+struct TbCrossEntropyFn : public Function<TbCrossEntropyFn> {
+    static Tensor forward(AutogradContext* ctx, const Tensor& logit_, const Tensor& label_) {
+        const Tensor logit = f32(logit_, "logit"), label = i64(label_, "label");
+        TORCH_CHECK_VALUE(label.dim() == 2, "label must be (T, B), got ", label.sizes());
+        TORCH_CHECK_VALUE(logit.dim() >= 1 && logit.size(-1) >= 1, "logit must be (*, N) with N >= 1, got ",
+                          logit.sizes());
+        const int64_t R = label.numel(), N = logit.size(-1);
+        TORCH_CHECK_VALUE(logit.numel() == R * N, "logit must hold T*B=", R, " rows of N=", N, ", got ",
+                          logit.sizes());
+        TORCH_CHECK_VALUE(label.device() == logit.device(), "logit and label must be on one device");
+        c10::cuda::CUDAGuard guard(logit.device());
+        Tensor out = torch::empty(label.sizes(), logit.options());
+        ck(hpc_rll_tb_cross_entropy_forward(fp(logit), ip(label), fpm(out), R, N, cur_stream()),
+           "hpc_rll_tb_cross_entropy_forward");
+        ctx->save_for_backward({logit, label});
+        return out;
+    }
+    static variable_list backward(AutogradContext* ctx, variable_list grads) {
+        const auto sv = ctx->get_saved_variables();
+        const Tensor &logit = sv[0], &label = sv[1];
+        if (!grads[0].defined()) return {Tensor(), Tensor()};
+        const Tensor g = f32(grads[0], "grad_out");
+        c10::cuda::CUDAGuard guard(logit.device());
+        Tensor gl = torch::empty_like(logit);
+        ck(hpc_rll_tb_cross_entropy_backward(fp(g), fp(logit), ip(label), fpm(gl), label.numel(), logit.size(-1),
+                                             cur_stream()),
+           "hpc_rll_tb_cross_entropy_backward");
+        return {gl, Tensor()};
+    }
+};
+
 // ------------------------------------------------------------------------------------------------ TD(lambda)
 struct TdLambdaFn : public Function<TdLambdaFn> {
     static Tensor forward(AutogradContext* ctx, const Tensor& value_, const Tensor& reward_, const OptTensor& weight_,
@@ -690,6 +766,15 @@ void register_fast_ops(pybind11::module& m) {
           [](const Tensor& r, const Tensor& v, bool save_mask) { return UpgoReturnsFn::apply(r, v, save_mask); },
           "UPGO returns with autograd (adjoint) in rewards and bootstrap_values; save_mask keeps the lambda mask "
           "the backward reads");
+    m.def("importance_weights",
+          [](const Tensor& t, const Tensor& b, const Tensor& a) {
+              const bool save = torch::GradMode::is_enabled() && (t.requires_grad() || b.requires_grad());
+              return ImportanceWeightsFn::apply(t, b, a, save);
+          },
+          "importance ratios pi(a) / mu(a) of two logits tensors, with autograd in both");
+    m.def("tb_cross_entropy",
+          [](const Tensor& logit, const Tensor& label) { return TbCrossEntropyFn::apply(logit, label); },
+          "log-softmax of the labelled action per (T, B) row, with autograd in logit");
     m.def("td_lambda",
           [](const Tensor& v, const Tensor& r, const OptTensor& w, double g, double l, int64_t gb) {
               return TdLambdaFn::apply(v, r, w, g, l, gb);

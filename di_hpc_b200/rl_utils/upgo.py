@@ -74,3 +74,28 @@ def upgo_returns(rewards, bootstrap_values):
     save_mask = torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad
                                                 for x in (rewards, bootstrap_values))
     return _ext.require().upgo_returns(rewards, bootstrap_values, save_mask)
+
+
+def tb_cross_entropy(logit, label, mask=None):
+    r"""
+    Overview:
+        The log-probability of the labelled action for every step of a ``(T, B)`` segment, as DI-engine's
+        ``tb_cross_entropy`` (hpc_rll/origin/upgo.py:7-18), i.e. ``-F.cross_entropy(logit, label, reduction='none')``
+        and UPGO's ``metric``.  Per row of ``N`` logits, with ``m = max x`` and ``s = Σ exp(x − m)``::
+
+            out = (x[a] − m) − log s
+
+        Differentiable in ``logit``: :math:`∂out/∂x[k] = 1[k=a] − p[k]`.  ``-inf`` (masked) logits are allowed and get
+        a gradient of exactly 0; a label outside ``[0, N)`` (PyTorch's ``ignore_index = −100`` included) or on a
+        masked entry is a precondition.  As in origin, only the 2-D label and ``mask=None`` are supported.
+    Arguments:
+        - logit (:obj:`torch.FloatTensor`): :math:`T·B` rows of :math:`N` logits, e.g. :math:`(T, B, N)`
+        - label (:obj:`torch.LongTensor`): :math:`(T, B)`
+        - mask: must be None
+    Returns:
+        - metric (:obj:`torch.FloatTensor`): :math:`(T, B)`
+    """
+    assert (len(label.shape) >= 2)
+    assert len(label.shape) == 2
+    assert mask is None
+    return _ext.require().tb_cross_entropy(logit, label)

@@ -95,3 +95,34 @@ def vtrace_nstep_return(clipped_rhos, clipped_cs, reward, bootstrap_values, gamm
                              "bootstrap_values only; pass %s.detach()" % (name, name))
     return _ext.require().vtrace_nstep_return(clipped_rhos, clipped_cs, reward, bootstrap_values, float(gamma),
                                               float(lambda_))
+
+
+def compute_importance_weights(target_output, behaviour_output, action, requires_grad=False):
+    r"""
+    Overview:
+        The importance-sampling ratios :math:`ρ = π(a) / μ(a)` of the chosen actions under the target and the
+        behaviour policy, as DI-engine's ``compute_importance_weights`` (hpc_rll/origin/vtrace.py:81-111).  Per row of
+        ``N`` logits, with ``m = max x`` and ``s = Σ exp(x − m)`` (the log-prob of ``torch.distributions.Categorical``)::
+
+            lp = x[a] − (m + log s)     per tensor        ρ = exp(lp_target − lp_behaviour)
+
+        One pass over both logits tensors; ρ is bit-identical to the ratios the fused ``VTrace`` loss forms for the
+        same rows.  Unlike ``Categorical`` with its default argument validation, nothing is checked on the host, so
+        the call never synchronises and can be captured in a CUDA graph.  ``-inf`` (masked) logits are allowed and
+        get a gradient of exactly 0; an action outside ``[0, N)`` or on a masked entry is a precondition.
+    Arguments:
+        - target_output (:obj:`torch.FloatTensor`): :math:`(*, N)`, logits of the target (current) policy, e.g.
+          :math:`(T, B, N)`
+        - behaviour_output (:obj:`torch.FloatTensor`): :math:`(*, N)`, logits of the behaviour policy, same shape
+        - action (:obj:`torch.LongTensor`): :math:`(*)`, the chosen actions
+        - requires_grad (:obj:`bool`): False (default) runs under ``torch.no_grad()`` and the result never requires
+          grad; True runs under ``torch.enable_grad()``, even inside an outer ``no_grad``, and gradients flow to
+          whichever logits tensor requires grad: :math:`∂ρ/∂x_t[k] = ρ·(1[k=a] − p_t[k])`,
+          :math:`∂ρ/∂x_b[k] = −ρ·(1[k=a] − p_b[k])`
+    Returns:
+        - rhos (:obj:`torch.FloatTensor`): :math:`(*)`
+    """
+    grad_context = torch.enable_grad() if requires_grad else torch.no_grad()
+    assert isinstance(action, torch.Tensor)
+    with grad_context:
+        return _ext.require().importance_weights(target_output, behaviour_output, action)

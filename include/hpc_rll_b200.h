@@ -49,7 +49,8 @@ extern "C" {
 #define HPC_RLL_OP_GAE_MOMENTS 9 /* workspace sizing only; tuning follows HPC_RLL_OP_GAE */
 #define HPC_RLL_OP_GAE_EPISODIC 10
 #define HPC_RLL_OP_LAMBDA_RETURNS 11
-#define HPC_RLL_OP_COUNT 12
+#define HPC_RLL_OP_IMPORTANCE_WEIGHTS 12 /* workspace sizing only (T*B = rows R); no tuning configs */
+#define HPC_RLL_OP_COUNT 13
 
 /* ---- library ------------------------------------------------------------------------------ */
 const char* hpc_rll_version(void);
@@ -59,7 +60,7 @@ uint64_t hpc_rll_launch_count(void);
 /* scratch bytes an op needs for sizes (T,B,N); N = action dim / n_atom / tau as relevant */
 size_t hpc_rll_workspace_bytes(int op, int64_t T, int64_t B, int64_t N);
 /* tuning/debug: force kernel configuration `cfg` for `op` (-1 = automatic); HPC_RLL_OP_LAMBDA_RETURNS accepts only
- * -1, 21 (look-back), 33 (wide) and 99 (generic) */
+ * -1, 21 (look-back), 33 (wide) and 99 (generic); HPC_RLL_OP_IMPORTANCE_WEIGHTS accepts none */
 int hpc_rll_debug_set_config(int op, int cfg);
 
 /* out[i] = a[0]*x[i] + b[0]*y[i]  (a, b DEVICE scalars; b and y may be NULL together: out = a[0]*x).  Glue for
@@ -194,6 +195,34 @@ int hpc_rll_upgo_returns_forward(const float* rewards, const float* bootstrap_va
                                  uint8_t* lambda_mask, int64_t T, int64_t B, void* stream);
 int hpc_rll_upgo_returns_backward(const float* grad_returns, const uint8_t* lambda_mask, float* grad_rewards,
                                   float* grad_bootstrap_values, int64_t T, int64_t B, void* stream);
+
+/* ---- importance weights and the time-batch cross entropy -----------------------------------------
+ * The per-row policy pieces of V-trace and UPGO as standalone ops (hpc_rll/origin/vtrace.py:81-111
+ * compute_importance_weights, hpc_rll/origin/upgo.py:7-18 tb_cross_entropy).  The logits tensors hold R contiguous
+ * rows of N floats, action / label R int64 indices in [0, N) (a precondition, not checked on the device).  Per row,
+ * with m = max_k x_k and s = sum_k exp(x_k - m):
+ *   importance weights (target, behaviour logits; the log-prob of torch.distributions.Categorical):
+ *     lp = x_a - (m + log s)  per tensor,   rho = expf(lp_target - lp_behaviour)
+ *     (bit-identical to the ratios hpc_rll_vtrace_forward forms for the same rows)
+ *   backward: grad_rho (R) -> grad_target_output, grad_behaviour_output (R,N); either pointer may be NULL (not
+ *     wanted), with c = grad_rho*rho (one rounded fp32 multiply) and p the row's softmax:
+ *     grad_target[k] = c*(1[k=a] - p_target[k]),   grad_behaviour[k] = -c*(1[k=a] - p_behaviour[k])
+ *     workspace: hpc_rll_workspace_bytes(HPC_RLL_OP_IMPORTANCE_WEIGHTS, R, 1, N) bytes
+ *   time-batch cross entropy (the log-softmax of F.cross_entropy; UPGO's `metric`):
+ *     out = (x_a - m) - log s
+ *   backward: grad_out (R) -> grad_logit (R,N),  grad_logit[k] = grad_out*(1[k=a] - p[k])
+ * -inf logits are clamped to -3e38 (their gradient is exactly 0).  R == 0 launches nothing and accepts NULL pointers;
+ * N must lie in [1, 2^30).  No call copies from the host. */
+int hpc_rll_importance_weights_forward(const float* target_output, const float* behaviour_output,
+                                       const int64_t* action, float* rho, int64_t R, int64_t N, void* stream);
+int hpc_rll_importance_weights_backward(const float* grad_rho, const float* target_output,
+                                        const float* behaviour_output, const int64_t* action, const float* rho,
+                                        float* grad_target_output, float* grad_behaviour_output, int64_t R, int64_t N,
+                                        void* workspace, size_t workspace_bytes, void* stream);
+int hpc_rll_tb_cross_entropy_forward(const float* logit, const int64_t* label, float* out, int64_t R, int64_t N,
+                                     void* stream);
+int hpc_rll_tb_cross_entropy_backward(const float* grad_out, const float* logit, const int64_t* label,
+                                      float* grad_logit, int64_t R, int64_t N, void* stream);
 
 /* test hook: the stage heights hpc_rll_gae_fwd_bwd_host would use for a (T,B) problem (host-only, no CUDA call);
  * writes up to `cap` entries, returns the number of stages */
